@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- training views/sec of the rasterizer hot path (BASELINE.json metric) on N GPUs of one node.
 
-  python bench.py --gpus 1 --steps 20 --warmup 5                       # our sm_100a path
+  python bench.py --gpus 1 --steps 20 --warmup 5                       # our sm_90a path
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W                         # view-parallel, one rank per GPU
   python bench.py --impl reference ...                                  # the reference's own CUDA kernels (oracle/_ref)
@@ -10,7 +10,8 @@ A "step" is one training view per rank through the public API: gaussian_renderer
 concatenation, rasterizer forward) -> L1 image loss -> backward to the six raw parameter leaves; for N > 1 the
 per-Gaussian gradients are then summed across ranks with ONE NCCL all-reduce (the path's only exchange).
 Workload = BASELINE.json configs[2]: 3M synthetic Gaussians, SH degree 3, 1920x1080, synthetic cameras.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR also writes what the last timed step computed (the loss and a fixed, seeded
+sample of 65 536 rows of every leaf gradient) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -38,7 +39,7 @@ def parse_args():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", choices=["ours", "reference", "reference-kernels"], default="ours",
-                    help="reference = the UNMODIFIED reference stack from baseline/_ref (its pybind extension built from RAST/setup.py, its "
+                    help="reference = the UNMODIFIED reference stack from oracle/_ref/stock (its pybind extension built from RAST/setup.py, its "
                          "gaussian_renderer.render, its GaussianModel, its l1_loss); reference-kernels = the reference's kernels behind our "
                          "own harness (oracle/_ref shim)")
     ap.add_argument("--mode", choices=["train", "distill"], default="train",
@@ -58,11 +59,13 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-exchange", action="store_true", help="DIAGNOSTIC ONLY (invalid for the metric): N>1 without any gradient exchange")
     ap.add_argument("--dense-allreduce", action="store_true", help="N>1: all-reduce the dense gradients instead of the compact SH exchange")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's loss and a seeded sample of its leaf gradients as DIR/<name>.npy")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks (B200_PROFILING.md recipe), sampled DURING the timed region
+# clocks, sampled DURING the timed region
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     """nvidia-smi polled every 50 ms from construction on; every line is stamped on arrival, and only the lines that arrived
@@ -185,9 +188,9 @@ def make_reference_render():
 
 def make_stock_reference(raw, dev):
     """The reference's own public path, UNMODIFIED (BASELINE.md section 2.1): `gaussian_renderer.render` + `scene.gaussian_model.GaussianModel`
-    + the pybind extension `diff_gaussian_rasterization._C` built from RAST/setup.py (rasterize_points.cu:46-299), all from baseline/_ref
-    (staged by baseline/stage_reference.py).  Returns (render_fn, gaussians, l1_loss, AdamW-factory) or None when it is not staged."""
-    ref = os.path.join(ROOT, "baseline", "_ref")
+    + the pybind extension `diff_gaussian_rasterization._C` built from RAST/setup.py (rasterize_points.cu:46-299), all from oracle/_ref/stock
+    (staged by oracle/stage_reference.py).  Returns (render_fn, gaussians, l1_loss, AdamW-factory) or None when it is not staged."""
+    ref = os.path.join(ROOT, "oracle", "_ref", "stock")
     tree = os.path.join(ref, "LightGaussian")
     ext = os.path.join(ref, "diff_gaussian_rasterization")
     if not (os.path.isfile(os.path.join(tree, "gaussian_renderer", "__init__.py")) and os.path.isdir(ext)
@@ -281,7 +284,7 @@ def main_distill(args, rank, world, dev):
     else:
         stock = make_stock_reference(scene["raw"], dev)
         if stock is None:
-            print(json.dumps({"impl": args.impl, "unavailable": "baseline/_ref (stock reference stack) is not staged"}))
+            print(json.dumps({"impl": args.impl, "unavailable": "oracle/_ref/stock (stock reference stack) is not staged"}))
             return 0
         render_fn, teacher, _ = stock
         import copy
@@ -292,7 +295,7 @@ def main_distill(args, rank, world, dev):
         torch_loss = make_torch_reference_loss(dev)
         loss_fn = torch_loss
         opt = torch.optim.AdamW([{"params": [getattr(student, n)], "lr": lr, "name": n} for n, lr in zip(names, lrs)], lr=0.0, eps=1e-15)
-        kind = "stock reference stack (baseline/_ref) + torch loss composition + torch.optim.AdamW"
+        kind = "stock reference stack (oracle/_ref/stock) + torch loss composition + torch.optim.AdamW"
     assert not student._features_rest.is_contiguous()
 
     def step(k):
@@ -535,7 +538,7 @@ def main():
             raise RuntimeError(f"gradient exchange self-check FAILED: {res}")
         return res
 
-    def timed(fn, steps, sampler=None):
+    def timed(fn, steps, sampler=None, after=None):
         barrier()
         torch.cuda.synchronize()
         if sampler:
@@ -546,6 +549,8 @@ def main():
             fn(args.warmup + s)
         e1.record()
         torch.cuda.synchronize()
+        if after:
+            after()
         clocks = None
         if sampler:
             sampler.end()
@@ -582,7 +587,30 @@ def main():
         step_resident(s)
     torch.cuda.synchronize()
     n0 = capi.launch_count() if args.impl == "ours" else 0
-    ms, clocks = timed(step_resident, args.steps, sampler)
+    dump = {}
+
+    def capture_outputs():
+        """what the last timed step computed: its loss and its leaf gradients, the latter as a fixed, seeded sample of rows"""
+        if not args.dump_outputs:
+            return
+        rows = torch.randperm(P, generator=torch.Generator().manual_seed(2024))[:min(P, 65536)].sort().values.to(dev)
+        dump["loss"] = last_loss[0].detach().double().reshape(1)
+        dump["sample_rows"] = rows.double()
+        for name, p_ in zip(("xyz", "features_dc", "features_rest", "scaling", "rotation", "opacity"), params):
+            dump["grad_" + name] = p_.grad.detach().reshape(P, -1).index_select(0, rows).float()
+        for k in dump:
+            dump[k] = dump[k].cpu().numpy()
+
+    last_loss = [None]
+
+    def step_resident_kept(step):
+        last_loss[0] = step_resident(step)
+
+    ms, clocks = timed(step_resident_kept, args.steps, sampler, after=capture_outputs)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k, a in dump.items():
+            np.save(os.path.join(args.dump_outputs, f"{k}.npy"), a)
     launches = (capi.launch_count() - n0) if args.impl == "ours" else 0
     views = args.steps * world
     value = views / (ms * 1e-3)
@@ -611,7 +639,7 @@ def main():
         if os.path.exists(peaks_path):
             peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
         else:
-            peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
         capi.profile_collect()
         capi.profile_enable(True)
         nprof = min(args.steps, 10)
@@ -660,14 +688,8 @@ def main():
         tot_ms = sum(v["ms_per_launch"] * v["launches"] for v in stages.values()) / nprof
         Bf = 12 * P + Pv * (32 + 12 * M) + 4 * P + 40 * Pv + 28 * R + 40 * R + 20 * N
         Bb = 20 * N + 40 * R + 88 * Pv + 12 * P + Pv * (32 + 12 * M) + P * (56 + 12 * M)
-        traffic = None   # DRAM bytes per launch of this kernel from the committed ncu --set full capture of the same workload
-        tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tpath) and (P, W, H) == (3_000_000, 1920, 1080):
-            for kname, bytes_ in json.load(open(tpath))["dram_bytes_per_launch"].items():
-                if kname.split("<")[0].replace("_raw", "") == top.replace("_raw", ""):
-                    traffic = bytes_      # ncu capture named in profiles/ncu_traffic.json["source"] (scripts/ncu_traffic.py)
         roofline = {"bound": "hbm", "kernel": top, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                    "traffic": traffic, "peak_source": peak_src,
+                    "peak_source": peak_src,
                     "share_of_native_time": stages[top]["ms_per_launch"] * stages[top]["launches"] / nprof / tot_ms,
                     "whole_view": {"alg_bytes": Bf + Bb, "native_ms_per_view": tot_ms,
                                    "achieved": (Bf + Bb) / (tot_ms * 1e-3) / 1e9, "frac": (Bf + Bb) / (tot_ms * 1e-3) / 1e9 / peak},
@@ -743,7 +765,7 @@ def main():
             if name == "fused_loss_and_adamw":
                 # device time of the N2/N3 kernels inside this iteration (library CUDA events), against the HBM peak
                 peak_rows = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]) \
-                    if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+                    if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
                 capi.profile_collect()
                 capi.profile_enable(True)
                 for s_ in range(5):
@@ -828,7 +850,7 @@ def main():
             vq_pass = {"fused_ms": t_o / 10, "torch_formulation_ms": t_t / 5, "assign_ms": ms_assign, "samples": nv, "codes": Kv, "dim": dv,
                        "fp32_kernel_only": fp32_only,
                        "what": "one importance-weighted EMA k-means iteration (VectorQuantize.forward in training mode); assign = operand split + "
-                               "tcgen05 coarse pass (bf16 hi/lo, K = 96, accumulators in TMEM) + exact FP32 rescore of the undecided rows; "
+                               "wgmma coarse pass (bf16 hi/lo, K = 96, FP32 accumulators in registers) + exact FP32 rescore of the undecided rows; "
                                "fp32_kernel_only = the FFMA kernel alone (2*n*K*d flops)"}
             del model_vq, xv, wv
         except Exception as ex:  # noqa: BLE001  (an auxiliary pass must never take the bench line down)
@@ -841,9 +863,9 @@ def main():
             cpu_baseline = {"value": v_cpu, "unit": UNIT, "cores": 1, "kind": "port",
                             "sample": f"1 view forward+backward of the same workload ({dt:.1f} s), oracle/lgo.c single thread; host has {os.cpu_count()} cores"}
         else:
-            how = ("its stock public path: gaussian_renderer.render + GaussianModel + the pybind extension built from RAST/setup.py (baseline/_ref)"
+            how = ("its stock public path: gaussian_renderer.render + GaussianModel + the pybind extension built from RAST/setup.py (oracle/_ref/stock)"
                    if kind == "reference" else
-                   "its kernels behind our harness (oracle/_ref: forward.cu/backward.cu/rasterizer_impl.cu compiled unmodified for sm_100a)")
+                   "its kernels behind our harness (oracle/_ref: forward.cu/backward.cu/rasterizer_impl.cu compiled unmodified for sm_90a)")
             cpu_baseline = {"value": value, "unit": UNIT, "cores": 0, "kind": "reference",
                             "sample": f"the reference has NO CPU implementation of this path: this arm times {how} on the same GPU, "
                                       f"same steps; host has {os.cpu_count()} cores"}

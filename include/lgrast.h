@@ -1,5 +1,5 @@
 /*
- * lgrast.h -- C-ABI of liblgrast.so, the B200 (sm_100a) rasterizer for LightGaussian's hot path.
+ * lgrast.h -- C-ABI of liblgrast.so, the H100 (sm_90a) rasterizer for LightGaussian's hot path.
  *
  * Drop-in boundary.  The four work entry points replace, one for one, the static C++ API the
  * reference's torch binding calls (RAST = submodules/compress-diff-gaussian-rasterization):
@@ -251,8 +251,8 @@ int lgr_compact_rows(int rows_out, const int32_t* src_row, int n_tensors, const 
  * lgr_vq_pack_indices / lgr_vq_unpack_indices: `bits` bits per index, most significant first, bytes filled from the high bit
  *   (dec2bin + np.packbits, vectree.py:120-125; np.unpackbits + bin2dec, vectree/utils.py:33-39); out has (n*bits+7)/8 bytes. */
 size_t lgr_vq_workspace_bytes(int64_t n);
-/* lgr_vq_assign for d <= 32 and n*K >= 2^20 runs the scores on the tensor cores (csrc/lgr_vq_tc.cuh: bf16 hi/lo split operands, tcgen05.mma,
- * accumulators in TMEM) and re-scores in exact FP32 only the rows whose two best codes are closer than the split's error bound; indices are
+/* lgr_vq_assign for d <= 32 and n*K >= 2^20 runs the scores on the tensor cores (csrc/lgr_vq_tc.cuh: bf16 hi/lo split operands, wgmma,
+ * FP32 accumulators in registers) and re-scores in exact FP32 only the rows whose two best codes are closer than the split's error bound; indices are
  * the same as the FP32 kernel's.  lgr_set_vq_mode(1) forces the FP32 kernel (A/B measurements).  The tensor-core path keeps a grow-only
  * device scratch (operand tiles) inside the library. */
 int lgr_set_vq_mode(int mode);

@@ -1,4 +1,4 @@
-"""lightgaussian_b200 -- B200 (sm_100a) implementation of LightGaussian's rasterizer hot path.
+"""lightgaussian_b200 -- H100 (sm_90a) implementation of LightGaussian's rasterizer hot path.
 
 Public surface (same names as the reference):
     GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians   (diff_gaussian_rasterization)

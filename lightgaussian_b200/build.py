@@ -1,5 +1,5 @@
-"""In-tree build of liblgrast.so (nvcc, sm_100a).  No JIT cache: the .so lives next to the sources so that
-it travels with the repository snapshot to the GPU box."""
+"""In-tree build of liblgrast.so (nvcc, sm_90a).  No JIT cache: the .so lives next to the sources, so a tree built once (on a
+machine without a GPU, too) runs anywhere it is copied."""
 from __future__ import annotations
 
 import os
@@ -15,7 +15,7 @@ SOURCES = ["lgrast.cu"]
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [os.path.join("..", "..", "include", "lgrast.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared",
 ]
@@ -25,7 +25,7 @@ HASH_PATH = LIB_PATH + ".srchash"
 
 
 def _source_hash() -> str:
-    """content hash of every source/header and the compiler flags (mtimes do not survive the snapshot copy to the GPU box)"""
+    """content hash of every source/header and the compiler flags (mtimes do not survive a copy of the tree)"""
     import hashlib
     h = hashlib.sha256(" ".join(NVCC_FLAGS).encode())
     for d in sorted(os.path.join(CSRC, s) for s in SOURCES + HEADERS):

@@ -31,7 +31,7 @@
 
 namespace {
 
-constexpr int BIN_V = 592;            // blocks of every count / scatter kernel = rows of the count matrix (148 SMs x 4)
+constexpr int BIN_V = 528;            // blocks of every count / scatter kernel = rows of the count matrix (132 SMs x 4)
 constexpr int DS_BITS = 11;
 constexpr int DS_BINS = 1 << DS_BITS;
 constexpr uint32_t BIN_NONE = 0xffffffffu;

@@ -2,7 +2,7 @@
 //
 // Forward math is written with explicitly rounded operations (LGR_MUL/ADD/FMA/...) in exactly the
 // operation order of the reference's compiled kernels (RAST/cuda_rasterizer/forward.cu:22-258,334-364
-// as nvcc 12.9 emits them for sm_100a), because the forward pass is full of discrete decisions that a
+// as nvcc 12.9 emits them for sm_90a), because the forward pass is full of discrete decisions that a
 // one-ulp difference can flip: the z<=0.2 cull, ceil() of the splat radius, int truncation of the tile
 // rectangle, the depth sort key, and the alpha / transmittance thresholds of the blend.  With the
 // order pinned, our forward output is bit-identical to the reference's on the same GPU.

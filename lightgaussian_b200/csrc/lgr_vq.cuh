@@ -110,7 +110,7 @@ void vq_launch_assign(int n, int d, int K, const float* x, const float* embed, u
     const int rows = RX * VQ_THREADS;
     const int row_tiles = (n + rows - 1) / rows;
     const int code_tiles = (K + VQ_TC - 1) / VQ_TC;
-    int splits = (4 * 148 * 3 + row_tiles - 1) / row_tiles;        // aim at >= 4 waves of 148 SMs x 3 resident blocks
+    int splits = (4 * 132 * 3 + row_tiles - 1) / row_tiles;        // aim at >= 4 waves of 132 SMs x 3 resident blocks
     splits = max(1, min(splits, code_tiles));
     const int tiles_per_split = (code_tiles + splits - 1) / splits;
     const int codes_per_split = tiles_per_split * VQ_TC;

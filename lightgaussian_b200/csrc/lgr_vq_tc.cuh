@@ -1,4 +1,4 @@
-// lgr_vq_tc.cuh -- nearest-code search of the VecTree k-means (vectree/vq.py:262-306: cdist + argmax) on the 5th-generation tensor cores.
+// lgr_vq_tc.cuh -- nearest-code search of the VecTree k-means (vectree/vq.py:262-306: cdist + argmax) on the Hopper tensor cores (wgmma).
 //
 // score[i][c] = |e_c|^2 - 2 x_i . e_c is a GEMM with a 27-long contraction (n = 80 000 samples x K = 8192 codes).  bf16 operands alone
 // would flip nearest-code decisions, and the parity contract is on the INDICES, so the kernel does a coarse pass on the tensor cores and an
@@ -7,12 +7,13 @@
 //   operands   x = x_hi + x_lo, e = e_hi + e_lo (two bf16 terms each, 16 bits of mantissa); the contraction is laid out as
 //              A' = [x_hi | x_hi | x_lo] (96 columns), B' = [e_hi | e_lo | e_hi], so ONE bf16 GEMM with K = 96 yields
 //              x_hi.e_hi + x_hi.e_lo + x_lo.e_hi with FP32 accumulation; the dropped terms are bounded by 3 * 2^-18 |x||e|.
-//   kernel     one CTA = 128 samples (UMMA M = 128) against all codes in tiles of 256 (UMMA N = 256): six tcgen05.mma (K = 16 each) per
-//              tile, issued by one thread, operands in shared memory as canonical K-major core-matrix tiles (no swizzle) that a prepare
-//              kernel wrote to global memory in exactly that order, so a tile arrives with ONE cp.async.bulk; accumulators in TMEM, two
-//              stages of 256 columns (all 512), so the MMAs of tile t+1 run under the epilogue of tile t.  Four epilogue warps read their
-//              32 TMEM lanes with tcgen05.ld (32 columns at a time), form score = |e|^2 - 2 acc and keep (best, second best, argmin);
-//              smallest index wins ties like the first-index argmax.
+//   kernel     one CTA = 128 samples against all codes in tiles of 256, operands in shared memory as canonical K-major core-matrix
+//              tiles (no swizzle) that a prepare kernel wrote to global memory in exactly that order, so a tile arrives with ONE
+//              cp.async.bulk (producer warp 8, two stages).  Warpgroups 0 and 1 each own 64 of the samples and compute a tile as two
+//              halves of 128 codes, six wgmma.m64n128k16 per half with the FP32 accumulators in registers; the epilogue of half 0 runs
+//              while the tensor cores work on half 1.  Each thread holds two rows x 32 columns of a half, forms score = |e|^2 - 2 acc and
+//              keeps (best, second best, argmin); the four lanes that share a row merge at the end.  Smallest index wins ties like the
+//              first-index argmax.
 //   decision   a row whose second-best score is within 2 * 1e-4 * |x_i| * max|e| of its best (>= 4x the error bound) is NOT decided here:
 //              its slot keeps ~0 and the exact FP32 kernel (vq_assign_kernel, lgr_vq.cuh) runs on the list of such rows (a few per cent).
 //              Every other row's argmin is provably the exact one.
@@ -26,7 +27,8 @@ constexpr int VT_DP = 32;          // padded feature dimension
 constexpr int VT_K = 3 * VT_DP;    // contraction length of the split GEMM
 constexpr int VT_A_BYTES = VT_M * VT_K * 2;
 constexpr int VT_B_BYTES = VT_N * VT_K * 2;
-constexpr int VT_THREADS = 192;    // warps 0-3 epilogue, warp 4 loads, warp 5 issues the MMAs and owns TMEM
+constexpr int VT_HN = 128;         // codes per wgmma (half a tile)
+constexpr int VT_THREADS = 288;    // warps 0-7 = two consumer warpgroups (64 samples each), warp 8 loads
 constexpr float VT_MARGIN = 2.0e-4f;
 
 __device__ __forceinline__ uint32_t vt_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -82,7 +84,7 @@ __global__ void __launch_bounds__(256) vt_prep_e_kernel(int K, int K_pad, int d,
     if (c < K) atomicMax(emax_bits, __float_as_uint(sqrtf(s)));
 }
 
-// ---- mbarrier / tcgen05 wrappers ----
+// ---- mbarrier / bulk-copy / wgmma wrappers ----
 __device__ __forceinline__ void vt_mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(vt_smem(bar)), "r"(count) : "memory"); }
 __device__ __forceinline__ void vt_mbar_expect_tx(uint64_t* bar, uint32_t bytes)
 {
@@ -97,10 +99,9 @@ __device__ __forceinline__ void vt_mbar_wait(uint64_t* bar, uint32_t parity)
                      : "=r"(ok)
                      : "r"(vt_smem(bar)), "r"(parity)
                      : "memory");
-        if (!ok && spin > (1u << 26)) {   // a protocol bug becomes an error, not a hung GPU
-            printf("lgrast: vq tensor-core pipeline barrier timed out (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
-            __trap();
-        }
+        // a protocol bug becomes a launch error, not a hung GPU (no printf here: a call inside the consumer loop would make ptxas
+        // serialise the wgmma pipeline)
+        if (!ok && spin > (1u << 26)) __trap();
     }
 }
 __device__ __forceinline__ void vt_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar)
@@ -111,31 +112,68 @@ __device__ __forceinline__ void vt_bulk_g2s(void* dst, const void* src, uint32_t
 }
 __device__ __forceinline__ uint64_t vt_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
 {
-    // UMMA shared-memory descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor): start address [0,14), leading byte offset [16,30),
-    // stride byte offset [32,46) -- all without their 4 LSBs --, version 1 at [46,48), layout type 0 = no swizzle at [61,64)
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32) |
-           (1ull << 46);
+    // wgmma shared-memory matrix descriptor: start address [0,14), leading byte offset [16,30) (core matrices adjacent in K), stride byte
+    // offset [32,46) (core matrices adjacent in M/N) -- all without their 4 LSBs --, base offset 0, layout type 0 = no swizzle at [62,64)
+    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32);
 }
-// instruction descriptor, kind::f16: D = F32 (1 << 4), A = B = BF16 (1 << 7, 1 << 10), both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-constexpr uint32_t VT_IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(VT_N >> 3) << 17) | ((uint32_t)(VT_M >> 4) << 24);
+__device__ __forceinline__ void vt_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void vt_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void vt_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void vt_mma(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
+// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T, bf16 operands (both K-major) from shared memory, FP32 accumulators in registers
+__device__ __forceinline__ void vt_wgmma(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
 {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(desc_a),
-                 "l"(desc_b), "r"(VT_IDESC), "r"(accumulate)
-                 : "memory");
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, "
+        "%29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, "
+        "%57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+          "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate)
+        : "memory");
 }
-__device__ __forceinline__ void vt_commit(uint64_t* bar)
+
+// (best, second best, argmin) of the columns a thread holds for one row.  Accumulator element i of an m64nNk16 wgmma sits in row
+// 16 * (warp % 4) + lane / 4 + 8 * ((i >> 1) & 1) and column 8 * (i >> 2) + 2 * (lane & 3) + (i & 1) of the warpgroup's 64 x N block.
+struct VtBest {
+    float best = 3.0e38f, second = 3.0e38f;
+    int arg = 0;
+    __device__ __forceinline__ void add(float sc, int c)   // columns arrive in increasing order: strict < keeps the smallest index
+    {
+        if (sc < best) { second = best; best = sc; arg = c; }
+        else if (sc < second) second = sc;
+    }
+    __device__ __forceinline__ void merge(float ob, float os, int oa)
+    {
+        if (ob < best || (ob == best && oa < arg)) { second = fminf(best, os); best = ob; arg = oa; }
+        else second = fminf(second, ob);
+    }
+};
+
+__device__ __forceinline__ void vt_epilogue(const float (&d)[64], const float* nrm, int cbase, int lane, VtBest& r0, VtBest& r1)
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(vt_smem(bar)) : "memory");
+#pragma unroll
+    for (int i = 0; i < 64; i++) {
+        const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        const float sc = fmaf(-2.0f, d[i], nrm[c]);
+        if ((i >> 1) & 1) r1.add(sc, cbase + c);
+        else r0.add(sc, cbase + c);
+    }
 }
 
 struct VtSmem {
     unsigned char a[VT_A_BYTES];         // 24 576 B
     unsigned char b[2][VT_B_BYTES];      // 2 x 49 152 B
     float norm[2][VT_N];
-    uint64_t full_a, full_b[2], acc_full[2], stage_free[2];
-    uint32_t tmem_base;
+    uint64_t full_a, full_b[2], stage_free[2];
 };
 
 __global__ void __launch_bounds__(VT_THREADS, 1)
@@ -152,21 +190,13 @@ vt_assign_kernel(int n, int K_pad, const unsigned char* __restrict__ A, const un
         vt_mbar_init(&sm.full_a, 1);
         for (int s = 0; s < 2; s++) {
             vt_mbar_init(&sm.full_b[s], 1);
-            vt_mbar_init(&sm.acc_full[s], 1);
-            vt_mbar_init(&sm.stage_free[s], 4);   // lane 0 of each epilogue warp
+            vt_mbar_init(&sm.stage_free[s], 8);   // lane 0 of each consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 5) {   // one warp allocates all 512 TMEM columns (2 accumulator stages of 256) and gives the permit back
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(vt_smem(&sm.tmem_base)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = sm.tmem_base;
 
-    if (warp == 4) {
+    if (warp == 8) {
         // ===== loads: the CTA's sample tile once, then the code tiles through two stages =====
         if (lane == 0) {
             vt_mbar_expect_tx(&sm.full_a, VT_A_BYTES);
@@ -180,82 +210,56 @@ vt_assign_kernel(int n, int K_pad, const unsigned char* __restrict__ A, const un
                 vt_bulk_g2s(sm.norm[s], norms + (size_t)t * VT_N, VT_N * 4, &sm.full_b[s]);
             }
         }
-    } else if (warp == 5) {
-        // ===== MMA issue: one thread, six K = 16 steps per 128 x 256 tile =====
-        if (lane == 0) {
-            vt_mbar_wait(&sm.full_a, 0);
-            const uint32_t a_addr = vt_smem(sm.a);
-            for (int t = 0; t < ntiles; t++) {
-                const int s = t & 1;
-                const uint32_t ph = (uint32_t)(t >> 1) & 1u;
-                vt_mbar_wait(&sm.stage_free[s], ph ^ 1u);   // the epilogue has drained accumulator stage s
-                vt_mbar_wait(&sm.full_b[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t b_addr = vt_smem(sm.b[s]);
+        return;
+    }
+
+    // ===== consumers: warpgroup g owns samples 64 g .. 64 g + 63 of the CTA's tile =====
+    const int g = warp >> 2;
+    const uint32_t a_addr = vt_smem(sm.a) + (uint32_t)g * (64 / 8) * 128u;
+    VtBest r0, r1;
+    float acc[2][64];
+    vt_mbar_wait(&sm.full_a, 0);
+    for (int t = 0; t < ntiles; t++) {
+        const int s = t & 1;
+        const uint32_t ph = (uint32_t)(t >> 1) & 1u;
+        vt_mbar_wait(&sm.full_b[s], ph);
+        const uint32_t b_addr = vt_smem(sm.b[s]);
+        vt_wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < VT_K / 16; k++) {
-                    const uint64_t da = vt_desc(a_addr + (uint32_t)k * 2u * (VT_M / 8) * 128u, (VT_M / 8) * 128u, 128u);
-                    const uint64_t db = vt_desc(b_addr + (uint32_t)k * 2u * (VT_N / 8) * 128u, (VT_N / 8) * 128u, 128u);
-                    vt_mma(tmem + (uint32_t)s * VT_N, da, db, k > 0 ? 1u : 0u);
-                }
-                vt_commit(&sm.acc_full[s]);   // arrives when the six MMAs have completed (implies fence::before_thread_sync)
-            }
-        }
-    } else {
-        // ===== epilogue: warp w owns TMEM lanes 32w .. 32w+31 = samples 32w + lane of the tile =====
-        const int row = blockIdx.x * VT_M + warp * 32 + lane;
-        float bestv = 3.0e38f, second = 3.0e38f;
-        int arg = 0;
-        for (int t = 0; t < ntiles; t++) {
-            const int s = t & 1;
-            const uint32_t ph = (uint32_t)(t >> 1) & 1u;
-            vt_mbar_wait(&sm.full_b[s], ph);     // the tile's |e|^2 (bulk copy, async proxy) is visible to this thread
-            vt_mbar_wait(&sm.acc_full[s], ph);   // ... and its accumulators are complete
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const float* nrm = sm.norm[s];
-#pragma unroll 1
-            for (int c0 = 0; c0 < VT_N; c0 += 32) {
-                uint32_t r[32];
-                const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(s * VT_N + c0);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
-                    "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-                      "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-                      "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-                      "=r"(r[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                const int cbase = t * VT_N + c0;
+        for (int h = 0; h < 2; h++) {
 #pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    const float sc = fmaf(-2.0f, __uint_as_float(r[j]), nrm[c0 + j]);
-                    if (sc < bestv) {
-                        second = bestv;
-                        bestv = sc;
-                        arg = cbase + j;
-                    } else if (sc < second) {
-                        second = sc;
-                    }
-                }
+            for (int k = 0; k < VT_K / 16; k++) {
+                const uint64_t da = vt_desc(a_addr + (uint32_t)k * 2u * (VT_M / 8) * 128u, (VT_M / 8) * 128u, 128u);
+                const uint64_t db = vt_desc(b_addr + (uint32_t)h * (VT_HN / 8) * 128u + (uint32_t)k * 2u * (VT_N / 8) * 128u, (VT_N / 8) * 128u, 128u);
+                vt_wgmma(acc[h], da, db, k > 0 ? 1u : 0u);
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) vt_mbar_arrive(&sm.stage_free[s]);
+            vt_wgmma_commit();
         }
+        vt_wgmma_wait<1>();   // half 0 is complete; half 1 still runs on the tensor cores
+        vt_epilogue(acc[0], sm.norm[s], t * VT_N, lane, r0, r1);
+        vt_wgmma_wait<0>();
+        vt_epilogue(acc[1], sm.norm[s] + VT_HN, t * VT_N + VT_HN, lane, r0, r1);
+        __syncwarp();
+        if (lane == 0) vt_mbar_arrive(&sm.stage_free[s]);   // this warp no longer reads stage s
+    }
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {   // the four lanes of a quad hold the same two rows
+        r0.merge(__shfl_xor_sync(0xffffffffu, r0.best, m), __shfl_xor_sync(0xffffffffu, r0.second, m), __shfl_xor_sync(0xffffffffu, r0.arg, m));
+        r1.merge(__shfl_xor_sync(0xffffffffu, r1.best, m), __shfl_xor_sync(0xffffffffu, r1.second, m), __shfl_xor_sync(0xffffffffu, r1.arg, m));
+    }
+    if ((lane & 3) < 2) {
+        const VtBest& r = (lane & 3) ? r1 : r0;
+        const int row = blockIdx.x * VT_M + 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * (lane & 3);
         if (row < n) {
             const float margin = 2.0f * VT_MARGIN * xnorm[row] * __uint_as_float(*emax_bits);
-            if (second - bestv > margin) {
-                best[row] = ((unsigned long long)vq_order_bits(bestv) << 32) | (unsigned)arg;
+            if (r.second - r.best > margin) {
+                best[row] = ((unsigned long long)vq_order_bits(r.best) << 32) | (unsigned)r.arg;
             } else {
                 best[row] = ~0ull;   // undecided here: the exact FP32 kernel fills it
                 undecided[atomicAdd(n_undecided, 1)] = row;
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 5) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
 }
 
 // the exact FP32 kernel of lgr_vq.cuh on a LIST of rows (the ones the tensor-core pass left undecided)

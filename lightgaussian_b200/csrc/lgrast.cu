@@ -1,4 +1,4 @@
-// lgrast.cu -- sm_100a kernels and the C-ABI (include/lgrast.h) of the B200 rasterizer.
+// lgrast.cu -- sm_90a kernels and the C-ABI (include/lgrast.h) of the H100 rasterizer.
 //
 // Pipeline per view (reference call order: RAST/cuda_rasterizer/rasterizer_impl.cu:198-337):
 //
@@ -37,6 +37,7 @@
 namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
+constexpr int LGR_SMS = 132;    // streaming multiprocessors of an H100 SXM: grid sizes of the grid-stride kernels
 constexpr int ACC_STRIDE = 12;  // floats per Gaussian in the backward accumulator record
 // record layout: 0..2 dL/dcolor rgb | 3 S0 | 4,5 S1x,S1y | 6,7,8 S2xx,S2xy,S2yy | 9..11 pad
 // with w = G * dL/dalpha per (pixel, Gaussian) pair and d = mean2D - pixel:  S0 = sum w, S1 = sum w*d, S2 = sum w*d*d^T.
@@ -1456,7 +1457,7 @@ int lgr_set_kback_mode(int mode)
 int lgr_set_vq_mode(int mode)
 {
     if (mode != 0 && mode != 1) {
-        g_last_error = "lgr_set_vq_mode: 0 = tcgen05 coarse pass + exact FP32 rescore (default), 1 = FP32 kernel only";
+        g_last_error = "lgr_set_vq_mode: 0 = tensor-core coarse pass + exact FP32 rescore (default), 1 = FP32 kernel only";
         return LGR_ERR_INVALID_ARG;
     }
     g_vq_mode = mode;
@@ -1744,7 +1745,7 @@ int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_pa
         else kback_zero_flag_kernel<true><<<(P + 255) / 256, 256, 0, stream>>>(z);
         LGR_LAUNCH_CHECK("kback_zero_flag_kernel", debug, stream);
         a.P = P;
-        const int blocks = std::min((P + KC_THREADS - 1) / KC_THREADS, 148 * 8);
+        const int blocks = std::min((P + KC_THREADS - 1) / KC_THREADS, LGR_SMS * 8);
         preprocess_backward_compact_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter);
         LGR_LAUNCH_CHECK("preprocess_backward_compact_kernel", debug, stream);
         return LGR_OK;
@@ -1860,7 +1861,7 @@ int lgr_backward_raw_sparse_pack_push(const lgr_view* v, int P, int M, const lgr
         sparse_flag_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, radii, geo.grad_acc, xb + L.bitmap, popc);
         LGR_CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, popc, xb + L.prefix, w32, stream));
         sparse_index_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, xb + L.bitmap, xb + L.prefix, idx, xb + L.hdr, v->campos);
-        if (world > 1) sparse_publish_kernel<<<148, 256, 0, stream>>>(push, self, L.rows);
+        if (world > 1) sparse_publish_kernel<<<LGR_SMS, 256, 0, stream>>>(push, self, L.rows);
         preprocess_backward_sparse_kernel<<<(P + SPK_THREADS - 1) / SPK_THREADS, SPK_THREADS, 0, stream>>>(a, idx, xb + L.hdr, push, L.rows);
     }
     LGR_LAUNCH_CHECK("preprocess_backward_sparse_kernel", debug, stream);
@@ -1918,7 +1919,7 @@ int lgr_peer_allreduce(float* const* peer_buffers, int rank, int world, size_t n
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     {
         ProfScope ps(ST_PEER_ALLREDUCE, stream);
-        peer_allreduce_kernel<<<148 * 2, 512, 0, stream>>>(pp, rank, world, n_floats / 4);
+        peer_allreduce_kernel<<<LGR_SMS * 2, 512, 0, stream>>>(pp, rank, world, n_floats / 4);
     }
     LGR_LAUNCH_CHECK("peer_allreduce_kernel", false, stream);
     return LGR_OK;
@@ -1934,7 +1935,7 @@ int lgr_multimem_allreduce(float* multicast_ptr, int rank, int world, size_t n_f
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     {
         ProfScope ps(ST_PEER_ALLREDUCE, stream);
-        multimem_allreduce_kernel<<<148 * 2, 512, 0, stream>>>(multicast_ptr, rank, world, n_floats / 4);
+        multimem_allreduce_kernel<<<LGR_SMS * 2, 512, 0, stream>>>(multicast_ptr, rank, world, n_floats / 4);
     }
     LGR_LAUNCH_CHECK("multimem_allreduce_kernel", false, stream);
     return LGR_OK;
@@ -2011,7 +2012,7 @@ int lgr_image_l1_forward(const float* img, const float* target, int C, int H, in
     const long long n = (long long)C * H * W;
     // never more blocks than the workspace of lgr_image_loss_workspace_bytes(C,H,W) holds partials for
     const long long cap = (long long)((W + LT - 1) / LT) * ((H + LT - 1) / LT) * C;
-    const int blocks = (int)std::max(1LL, std::min({cap, (n / 4 + 255) / 256, 148LL * 8}));
+    const int blocks = (int)std::max(1LL, std::min({cap, (n / 4 + 255) / 256, (long long)LGR_SMS * 8}));
     {
         ProfScope ps(ST_LOSS_FWD, stream);
         image_l1_forward_kernel<<<blocks, 256, 0, stream>>>(img, target, n, (float2*)workspace);
@@ -2187,7 +2188,7 @@ int lgr_vq_assign(int n, int d, int K, const float* x, const float* embed, const
     if (n == 0) return LGR_OK;
     unsigned long long* best = static_cast<unsigned long long*>(workspace);
     if (g_vq_mode == 0 && d <= VT_DP && (long long)n * K >= (1ll << 20)) {
-        // coarse pass on the tensor cores (tcgen05, lgr_vq_tc.cuh) + exact FP32 rescore of the undecided rows
+        // coarse pass on the tensor cores (wgmma, lgr_vq_tc.cuh) + exact FP32 rescore of the undecided rows
         const int n_pad = (n + VT_M - 1) / VT_M * VT_M, K_pad = (K + VT_N - 1) / VT_N * VT_N;
         const size_t oA = 0, oB = oA + vt_align((size_t)(n_pad / VT_M) * VT_A_BYTES), oN = oB + vt_align((size_t)(K_pad / VT_N) * VT_B_BYTES),
                      oX = oN + vt_align((size_t)K_pad * 4), oC = oX + vt_align((size_t)n_pad * 4), oL = oC + 1024, total = oL + vt_align((size_t)n * 4);

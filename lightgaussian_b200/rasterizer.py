@@ -491,9 +491,8 @@ def _symm_exchange(device, P, world, group):
         _symm_cache.pop(key, None)
         del cur
         xb, ok = None, 1
-        # Measured on 2 and 4 B200s (DESIGN.md section 6): NCCL's all-reduce is as fast or faster than our peer-memory and
-        # NVLS multimem kernels for this 132 MB payload once the rebuild kernel competes for HBM, so NCCL is the default;
-        # LGR_EXCHANGE_REDUCE=peer|multimem selects ours.
+        # NCCL's all-reduce is the default: for this 132 MB payload the rebuild kernel competes for HBM with whichever reduction
+        # runs, so our peer-memory and NVLS multimem kernels have no bandwidth to gain; LGR_EXCHANGE_REDUCE=peer|multimem selects ours.
         if os.environ.get("LGR_EXCHANGE_REDUCE", "nccl") == "nccl":
             ok = 0
         else:
@@ -648,8 +647,8 @@ def _backward_raw_sparse(xs, rs, num_rendered, grad_out_color, xyz, dc, rest, sc
 
 def _exchange_chunks(P):
     """[(first, count)] ranges of Gaussians, boundaries at multiples of 256.  LGR_EXCHANGE_CHUNKS ranges; default 1 = one all-reduce
-    after the whole K7+K8: measured on 2 B200s, 2 / 4 ranges were SLOWER (624 / 581 vs 672 views/s): the NCCL kernels of the earlier ranges
-    take SMs and HBM bandwidth from the ranges still being computed (K7+K8 0.20 -> 0.38 ms) and the link was not idle to begin with."""
+    after the whole K7+K8: with more ranges the NCCL kernels of the earlier ranges take SMs and HBM bandwidth from the ranges still
+    being computed."""
     import os
     n = max(1, int(os.environ.get("LGR_EXCHANGE_CHUNKS", "1")))
     blocks = (P + 255) // 256

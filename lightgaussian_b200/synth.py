@@ -1,6 +1,6 @@
 """Deterministic synthetic scenes and cameras (SURVEY.md section 8d) for tests and bench.py.
 
-There is no dataset or checkpoint on the GPU box, so every measurement uses a seeded random
+No dataset or checkpoint ships with the project, so every measurement uses a seeded random
 Gaussian cloud and cameras on a Fibonacci sphere.  Camera matrices follow the reference's
 convention exactly (scene/cameras.py:70-85, utils/graphics_utils.py:38-77): `world_view_transform`
 and `full_proj_transform` are stored TRANSPOSED (row-vector convention), `camera_center` is row 3

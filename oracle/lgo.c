@@ -10,8 +10,8 @@
  * Parity pin: the reference ships no tests or golden vectors for this path
  * (SURVEY.md section 4).  The oracle is pinned instead by
  *   (1) tests/golden/ref_*.npz -- outputs of the reference's own CUDA kernels, compiled
- *       unmodified from /root/reference by oracle/Makefile into oracle/_ref and executed
- *       on a B200 (generator: tests/golden/make_ref_golden.py);
+ *       unmodified from the reference checkout by oracle/Makefile into oracle/_ref and
+ *       executed on the GPU (generator: tests/golden/make_ref_golden.py);
  *   (2) tests/golden/pyref_*.npz -- outputs of the reference's Python sub-steps
  *       (utils/sh_utils.py eval_sh) imported on CPU (generator: make_pyref_golden.py);
  *   (3) a finite-difference check of the backward pass against the double-precision
@@ -19,7 +19,7 @@
  *
  * Arithmetic order.  The forward functions reproduce the reference's *compiled*
  * float operation order (which multiply-adds are fused) as read from the SASS that
- * nvcc 12.9 emits for RAST/cuda_rasterizer/forward.cu on sm_100a, so that every
+ * nvcc 12.9 emits for RAST/cuda_rasterizer/forward.cu on sm_90a, so that every
  * discrete decision (near-plane cull, radius ceil, tile rectangle truncation, depth
  * sort key) matches the GPU bit for bit.  sqrt, division and reciprocal are IEEE
  * correctly rounded on both sides.  The one exception is exp(): the GPU uses

@@ -2,9 +2,9 @@
 //
 // A plain C-ABI around the reference's own, unmodified CudaRasterizer::Rasterizer static API
 // (declared in RAST/cuda_rasterizer/rasterizer.h:20-113).  oracle/Makefile compiles the
-// reference's forward.cu / backward.cu / rasterizer_impl.cu from /root/reference together with
+// reference's forward.cu / backward.cu / rasterizer_impl.cu from the reference checkout together with
 // this file into oracle/_ref/libref_rasterizer.so.  It exists so that
-//   * tests can compare our kernels with the real reference kernels on the same B200, and
+//   * tests can compare our kernels with the real reference kernels on the same GPU, and
 //   * bench.py --impl reference can time the reference's CUDA path next to ours,
 // without torch/pybind in between (the reference's torch binding, RAST/rasterize_points.cu,
 // only allocates tensors and forwards raw pointers to this same API).

@@ -1,6 +1,5 @@
 """SASS mnemonic counts per kernel of the built library (cuobjdump -sass): the static evidence that TMA bulk copies (UBLKCP), mbarriers
-(SYNCS), tcgen05 (UTCHMMA = tcgen05.mma kind::f16, LDTM = tcgen05.ld, UTCBAR = tcgen05.commit, UTCATOMSWS = tcgen05.alloc) are in the kernels
-that claim them.  usage: python scripts/sass_evidence.py > profiles/<round>_sass_evidence.txt"""
+(SYNCS) and warpgroup MMAs (HGMMA = wgmma.mma_async) are in the kernels that claim them.  usage: python scripts/sass_evidence.py"""
 import collections
 import os
 import re
@@ -9,7 +8,7 @@ import subprocess
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "lightgaussian_b200", "_lib", "liblgrast.so")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
-KEYS = ["UTCHMMA", "LDTM", "UTCBAR", "UTCATOMSWS", "UBLKCP", "SYNCS", "LDG.E.128", "REDG", "ATOMS", "MUFU", "LDS.128", "VOTE", "FFMA"]
+KEYS = ["HGMMA", "UBLKCP", "SYNCS", "LDG.E.128", "REDG", "ATOMS", "MUFU", "LDS.128", "VOTE", "FFMA"]
 cur, counts, total = None, collections.OrderedDict(), {}
 for line in out.splitlines():
     m = re.search(r"Function : (\S+)", line)
@@ -27,8 +26,8 @@ for line in out.splitlines():
         for k in KEYS:
             if op.startswith(k):
                 counts[cur][k] += 1
-print("# SASS mnemonic counts per kernel (cuobjdump -sass, sm_100a): UTCHMMA = tcgen05.mma kind::f16, LDTM = tcgen05.ld, UTCBAR = tcgen05.commit,")
-print("# UTCATOMSWS = tcgen05.alloc/dealloc, UBLKCP = cp.async.bulk (TMA bulk copy), SYNCS = mbarrier, REDG = fire-and-forget global reductions")
+print("# SASS mnemonic counts per kernel (cuobjdump -sass, sm_90a): HGMMA = wgmma.mma_async, UBLKCP = cp.async.bulk (TMA bulk copy),")
+print("# SYNCS = mbarrier, REDG = fire-and-forget global reductions")
 for name, c in counts.items():
     short = re.sub(r"^_ZN\d+_GLOBAL__N__[0-9a-f]+_\d+_lgrast_cu_[0-9a-f]+", "", name)[:72]
     print(f"{short:72s} " + " ".join(f"{k} {c[k]:3d}" for k in KEYS) + f" total {total[name]:5d}")

@@ -1,6 +1,6 @@
 """Generates tests/golden/pyref_sh.npz by IMPORTING the reference's own Python SH evaluator
 (/root/reference/utils/sh_utils.py:57-120, the `convert_SHs_python` path of gaussian_renderer/__init__.py:79-96)
-on CPU.  Run in the build container (needs /root/reference); the .npz is committed.
+on CPU.  Needs the reference checkout; the .npz is committed.
 
     python tests/golden/make_pyref_golden.py
 """

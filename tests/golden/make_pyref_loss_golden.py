@@ -1,6 +1,6 @@
 """Generates tests/golden/pyref_loss.npz by IMPORTING the reference's own loss module (/root/reference/utils/loss_utils.py)
 on CPU: l1_loss, ssim and the autograd gradient of the training loss (1-l)*l1 + l*(1-ssim) (prune_finetune.py:160-164).
-Run in the build container:  python tests/golden/make_pyref_loss_golden.py"""
+Needs the reference checkout:  python tests/golden/make_pyref_loss_golden.py"""
 import importlib.util
 import os
 

@@ -2,10 +2,11 @@
 (oracle/_ref/libref_rasterizer.so, compiled unmodified from /root/reference by oracle/Makefile) on the seeded
 inputs of tests/util.py:CONFIGS.  Needs a GPU:
 
-    gpurun -- 'python tests/golden/make_ref_golden.py gpurun_out/golden'    # then copy the .npz into tests/golden/
+    python tests/golden/make_ref_golden.py <out dir>    # then copy the .npz into tests/golden/
 
 The inputs are NOT stored (they are regenerated from the seed); a checksum guards against generator drift.
 """
+import hashlib
 import os
 import sys
 import zlib
@@ -33,7 +34,7 @@ def main(out_dir):
         d = dict(input_crc=np.uint32(checksum(act, dpix)), num_rendered=np.int64(fwd["num_rendered"]), color=fwd["color"],
                  radii=fwd["radii"], final_T=fwd["final_T"], n_contrib=fwd["n_contrib"], point_list=fwd["point_list"],
                  ranges=fwd["ranges"], ref_racy_count=cnt["gaussians_count"], ref_racy_score=cnt["important_score"],
-                 count_color=cnt["color"])
+                 count_color_sha256=np.frombuffer(hashlib.sha256(np.ascontiguousarray(cnt["color"]).tobytes()).digest(), np.uint8))
         for k, v in fwd["geom"].items():
             d["geom_" + k] = v
         for k, v in fwd["grads"].items():
@@ -44,4 +45,4 @@ def main(out_dir):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gpurun_out", "golden"))
+    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "golden_out"))

@@ -2,7 +2,7 @@
 vectree/vectree.py): per-iteration states of the importance-weighted EMA k-means (VectorQuantize.forward with weight, then the
 k_expire replacement of vectree.py:203-205), the final encode, and the on-disk codec (extreme_saving/*.npz written by
 Quantization.fully_vq_reformat, read back by load_vqgaussian).
-Run in the build container:  python tests/golden/make_vq_golden.py"""
+Needs the reference checkout:  python tests/golden/make_vq_golden.py"""
 import os
 import sys
 import tempfile
@@ -90,5 +90,6 @@ idx = rng.integers(0, 2 ** 13, 1001)
 out["codec_idx"] = idx
 out["codec_packed"] = np.packbits(ref_utils.dec2bin(torch.from_numpy(idx), 13).bool().numpy().reshape(-1))
 out["codec_roundtrip"] = ref_utils.bin2dec(torch.from_numpy(np.unpackbits(out["codec_packed"])[:1001 * 13].reshape(1001, 13)).float(), 13).long().numpy()
+assert np.array_equal(out["full_feats"][:, 6:6 + D], out.pop("feats_sh"))   # the readers take it from full_feats (keeps the file < 1 MB)
 np.savez_compressed(os.path.join(HERE, "pyref_vq.npz"), **out)
 print("ok", {k: v.shape for k, v in out.items() if k.startswith(("file_", "all_", "deq"))})

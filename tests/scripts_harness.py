@@ -1,10 +1,10 @@
-"""Harness for running the reference's scripts UNMODIFIED on the GPU box (tests/test_gpu_scripts.py).
+"""Harness for running the reference's scripts UNMODIFIED on a GPU (tests/test_gpu_scripts.py).
 
-Two import stacks over the same verbatim copy of the reference's Python tree (baseline/_ref/LightGaussian, staged by
-baseline/stage_reference.py in the build container; /root/reference does not exist on the GPU box):
+Two import stacks over the same verbatim copy of the reference's Python tree (oracle/_ref/stock/LightGaussian, staged by
+oracle/stage_reference.py when build() finds the reference checkout):
 
-  ours   PYTHONPATH = <repo>/dropin : <repo> : baseline/_ref/LightGaussian          -> our rasterizer / loss / optimizer
-  stock  PYTHONPATH = baseline/_ref : baseline/_ref/shims : baseline/_ref/LightGaussian
+  ours   PYTHONPATH = <repo>/dropin : <repo> : oracle/_ref/stock/LightGaussian          -> our rasterizer / loss / optimizer
+  stock  PYTHONPATH = oracle/_ref/stock : oracle/_ref/stock/shims : oracle/_ref/stock/LightGaussian
                                                                                      -> the reference's own pybind extension (built
                                                                                         from RAST/setup.py), gaussian_renderer, loss, AdamW
 
@@ -22,7 +22,7 @@ import sys
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REFDIR = os.path.join(ROOT, "baseline", "_ref")
+REFDIR = os.path.join(ROOT, "oracle", "_ref", "stock")
 TREE = os.path.join(REFDIR, "LightGaussian")
 HELPERS = os.path.join(ROOT, "tests", "helpers")
 
@@ -30,12 +30,12 @@ HELPERS = os.path.join(ROOT, "tests", "helpers")
 def stacks_available() -> str | None:
     """None when both stacks can run, else the reason."""
     if not os.path.isfile(os.path.join(TREE, "prune_finetune.py")):
-        return "baseline/_ref/LightGaussian is not staged (run baseline/stage_reference.py in the build container)"
+        return "oracle/_ref/stock/LightGaussian is not staged (oracle/stage_reference.py needs the reference checkout)"
     ext = os.path.join(REFDIR, "diff_gaussian_rasterization")
     if not (os.path.isdir(ext) and any(f.startswith("_C") and f.endswith(".so") for f in os.listdir(ext))):
-        return "baseline/_ref/diff_gaussian_rasterization (the reference's own extension) is not built"
+        return "oracle/_ref/stock/diff_gaussian_rasterization (the reference's own extension) is not built"
     if not os.path.isdir(os.path.join(REFDIR, "shims")):
-        return "baseline/_ref/shims is not staged"
+        return "oracle/_ref/stock/shims is not staged"
     return None
 
 

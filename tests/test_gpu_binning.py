@@ -70,7 +70,7 @@ def test_backward_after_estimated_and_repeated_forward():
             assert util.rel_inf(got["grads"][k], ref["grads"][k]) <= 1e-4, k     # same kernels, atomics reorder the sums
 
 
-needs_ref = pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs /root/reference)")
+needs_ref = pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs the reference checkout)")
 
 
 @needs_ref

@@ -61,7 +61,7 @@ def test_backward_is_linear_in_the_pixel_gradient(big):
         assert np.all(g1[k][cul] == 0), k
 
 
-@pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs /root/reference)")
+@pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs the reference checkout)")
 def test_full_size_parity_with_reference_kernels(big):
     act, view, dpix = big
     ours = run_ours(view, act, dL_dpix=dpix)
@@ -89,7 +89,7 @@ def test_full_size_parity_with_reference_kernels(big):
     assert 0.0 <= lost < 1.0 and np.isfinite(rho)
 
 
-@pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs /root/reference)")
+@pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs the reference checkout)")
 def test_bench_config_3m_1080p_parity_with_reference_kernels():
     """The exact bench.py workload (BASELINE.json configs[2] scene: 3M Gaussians, SH degree 3, 1920x1080, camera 0 of the bench's
     16): forward bit-identical to the reference's kernels, gradients to 1e-3."""

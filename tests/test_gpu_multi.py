@@ -1,4 +1,4 @@
-"""2-GPU (NCCL) check of the view-parallel path on real renders; skipped on a single-GPU box."""
+"""2-GPU (NCCL) check of the view-parallel path on real renders; skipped on a machine with one GPU."""
 import os
 import socket
 

@@ -1,6 +1,6 @@
-"""GPU parity tests: our sm_100a path (through the C-ABI) against
+"""GPU parity tests: our sm_90a path (through the C-ABI) against
   (a) the CPU oracle (oracle/lgo.c), stage by stage, and
-  (b) the reference's own CUDA kernels compiled into oracle/_ref (when that library travelled to the box).
+  (b) the reference's own CUDA kernels compiled into oracle/_ref (where oracle/Makefile could build it).
 
 Tolerances (BASELINE.json north_star): rendered RGB 1e-4 abs, gradients 1e-3 rel, significance exact.
 Forward comparisons against the reference kernels are expected to be BIT-EXACT because lgr_math.cuh pins
@@ -144,7 +144,7 @@ def test_precomputed_inputs_vs_oracle():
 # ------------------------------------------------------------------------------------------------
 # against the reference's own kernels (oracle/_ref), same GPU
 # ------------------------------------------------------------------------------------------------
-needs_ref = pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs /root/reference)")
+needs_ref = pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref/libref_rasterizer.so not built (needs the reference checkout)")
 
 
 @needs_ref

@@ -13,7 +13,8 @@ from lightgaussian_b200 import vectree as vt
 from oracle import vq_oracle as vo
 
 pytestmark = pytest.mark.gpu
-G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pyref_vq.npz"))
+G = dict(np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pyref_vq.npz")))
+G["feats_sh"] = G["full_feats"][:, 6:33]   # the VQ'd SH columns of the full feature rows (stored once)
 N, D, K, CHUNK, ITERS, KEXP = (int(v) for v in G["cfg"])
 
 
@@ -175,7 +176,7 @@ def test_cpu_tensors_are_refused():
 
 
 def test_tensor_core_search_equals_the_fp32_kernel_at_full_size():
-    """80 000 x 8192 x 27 (vectree/vq.py's chunk): the tcgen05 coarse pass + exact rescore of the undecided rows must return the FP32
+    """80 000 x 8192 x 27 (vectree/vq.py's chunk): the tensor-core (wgmma) coarse pass + exact rescore of the undecided rows must return the FP32
     kernel's indices -- both kernels break exact ties towards the smaller index; rows whose two best codes differ by less than the fp32
     rounding of the expansion may legitimately differ and are checked in float64"""
     from lightgaussian_b200 import capi

@@ -5,7 +5,8 @@ import numpy as np
 
 from oracle import vq_oracle as vo
 
-G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pyref_vq.npz"))
+G = dict(np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pyref_vq.npz")))
+G["feats_sh"] = G["full_feats"][:, 6:33]   # the VQ'd SH columns of the full feature rows (stored once)
 N, D, K, CHUNK, ITERS, KEXP = (int(v) for v in G["cfg"])
 
 
@@ -46,7 +47,7 @@ def test_on_disk_format_and_dequantize():
     bits = int(np.log2(K))
     np.testing.assert_array_equal(vo.pack_indices(G["all_indice"][vq_mask], bits), G["file_vq_indexs"])
     np.testing.assert_array_equal(np.packbits(G["non_vq_mask"]), G["file_non_vq_mask"])
-    files = {k[5:]: G[k] for k in G.files if k.startswith("file_") and k != "file_metadata"}
+    files = {k[5:]: G[k] for k in G if k.startswith("file_") and k != "file_metadata"}
     np.testing.assert_array_equal(vo.dequantize(files, G["file_metadata"]), G["dequantized"])
     # the encode the files came from: nearest code of the (float32) final codebook, features rounded through fp16
     idx, gap = vo.assign(G["feats_sh"], G[f"it{ITERS - 1}_embed_after_replace"][0])
