@@ -11,6 +11,7 @@ import pytest
 
 from tests import util
 from tests.util import CONFIGS, make_config, run_ours, run_ref, rel_inf, rel_l2, oracle_from_geometry, assert_elementwise
+from tests.util import oracle_backward_on_our_state
 from oracle.lgo import Oracle
 
 pytestmark = pytest.mark.gpu
@@ -21,21 +22,6 @@ GRAD_TOL = 1e-3    # rel, north_star
 
 def _clamp_bits(clamped3):
     return (clamped3[:, 0].astype(np.uint8) | (clamped3[:, 1].astype(np.uint8) << 1) | (clamped3[:, 2].astype(np.uint8) << 2))
-
-
-def _oracle_backward_on_our_state(o, view, act, ours, dpix, colors=None, cov=None):
-    geom = ours["geom"]
-    P = act["means3D"].shape[0]
-    clamped3 = np.stack([(geom["clamped_bits"] >> c) & 1 for c in range(3)], axis=1).astype(np.uint8)
-    col = geom["rgb"] if colors is None else colors
-    g2 = o.blend_backward(view, P, ours["ranges"], ours["point_list"], geom["means2D"], geom["conic_opacity"], col,
-                          ours["final_T"], ours["n_contrib"], dpix)
-    g3 = o.preprocess_backward(view, act["means3D"], ours["radii"], clamped3, geom["cov3D"] if cov is None else cov,
-                               g2["dL_dmean2D"], g2["dL_dconic"], g2["dL_dcolor"],
-                               shs=None if colors is not None else act["shs"],
-                               scales=None if cov is not None else act["scales"],
-                               rotations=None if cov is not None else act["rotations"])
-    return g2, g3
 
 
 @pytest.mark.parametrize("name", list(CONFIGS))
@@ -91,7 +77,7 @@ def test_backward_vs_oracle(name):
     act, view, dpix = make_config(name)
     ours = run_ours(view, act, dL_dpix=dpix)
     o = Oracle()
-    g2, g3 = _oracle_backward_on_our_state(o, view, act, ours, dpix)
+    g2, g3 = oracle_backward_on_our_state(o, view, act, ours, dpix)
     mine = ours["grads"]
     checks = {
         "dL_dmeans2D": (mine["dL_dmeans2D"][:, :2], g2["dL_dmean2D"]),
@@ -132,7 +118,7 @@ def test_precomputed_inputs_vs_oracle():
     ref = oracle_from_geometry(o, view, ours["geom"])
     err = np.abs(ours["color"] - ref["color"]).max(axis=0)
     assert err[~ref["fragile"]].max() <= RGB_TOL
-    g2, g3 = _oracle_backward_on_our_state(o, view, act, ours, dpix, colors=colors, cov=cov)
+    g2, g3 = oracle_backward_on_our_state(o, view, act, ours, dpix, colors=colors, cov=cov)
     mine = ours["grads"]
     for a, b, k in ((mine["dL_dcolors"], g2["dL_dcolor"], "dL_dcolors"), (mine["dL_dcov3D"], g3["dL_dcov3D"], "dL_dcov3D"),
                     (mine["dL_dmeans3D"], g3["dL_dmeans3D"], "dL_dmeans3D"), (mine["dL_dopacity"].reshape(-1), g2["dL_dopacity"], "dL_dopacity")):
@@ -226,7 +212,7 @@ def test_config_c1_10k_400x400_vs_reference_kernels(cam):
     culled = run_ours(view, scene["act"])                       # the product default (exact tile culling): same image
     np.testing.assert_array_equal(culled["color"], ref["color"])
     # arbiter for the per-element check: the float64 oracle's backward on the (bit-identical) forward state
-    g2, g3 = _oracle_backward_on_our_state(Oracle(double=True), view, scene["act"], ours, dpix)
+    g2, g3 = oracle_backward_on_our_state(Oracle(double=True), view, scene["act"], ours, dpix)
     exact = {"dL_dmeans2D": np.concatenate([g2["dL_dmean2D"], np.zeros((g2["dL_dmean2D"].shape[0], 1))], axis=1), "dL_dcolors": g2["dL_dcolor"],
              "dL_dopacity": g2["dL_dopacity"], "dL_dmeans3D": g3["dL_dmeans3D"], "dL_dcov3D": g3["dL_dcov3D"], "dL_dsh": g3["dL_dsh"],
              "dL_dscales": g3["dL_dscales"], "dL_drotations": g3["dL_drotations"]}

@@ -30,16 +30,35 @@ def _ties_only(x, embed, ours, ref):
     return bool(np.all(np.abs(da - db) <= tol))
 
 
-@pytest.mark.parametrize("n,d,K_", [(1, 27, 64), (257, 27, 8192), (5000, 48, 512), (3000, 3, 7), (999, 64, 100), (70000, 27, 300)])
+@pytest.mark.parametrize("n,d,K_", [(1, 27, 64), (257, 27, 8192), (5000, 48, 512), (3000, 3, 7), (999, 64, 100), (70000, 27, 300),
+                                    # the tensor-core route (d <= 32, n*K >= 2^20) at ragged n (not a multiple of 128) and K (not a
+                                    # multiple of 256): the contraction zero-padded to 32 (d < 27, d = 28..31) and unpadded (d = 32)
+                                    (4097, 1, 300), (20000, 8, 1000), (3001, 16, 700), (9000, 28, 257), (9000, 31, 257),
+                                    (12345, 32, 4096)])
 def test_assign_matches_oracle(n, d, K_):
+    from lightgaussian_b200 import capi
     rng = np.random.default_rng(n + d)
     x = rng.standard_normal((n, d)).astype(np.float32)
     e = rng.standard_normal((K_, d)).astype(np.float32) * 1.5
-    idx = vt.vq_assign(torch.from_numpy(x).cuda(), torch.from_numpy(e).cuda()).cpu().numpy()
+    xt, et = torch.from_numpy(x).cuda(), torch.from_numpy(e).cuda()
+    n0 = capi.launch_count()
+    idx = vt.vq_assign(xt, et).cpu().numpy()
+    launches = capi.launch_count() - n0
     ref, _ = vo.assign(x, e)
     assert idx.min() >= 0 and idx.max() < K_
     assert _ties_only(x, e, idx, ref)
     assert (idx != ref).mean() < 1e-3
+    capi.set_vq_mode(1)                   # the FP32 kernel only
+    try:
+        n0 = capi.launch_count()
+        idx_fp32 = vt.vq_assign(xt, et).cpu().numpy()
+        launches_fp32 = capi.launch_count() - n0
+    finally:
+        capi.set_vq_mode(0)
+    assert _ties_only(x, e, idx_fp32, ref)
+    # lgr_vq_assign takes the tensor-core coarse pass + rescore (more launches than the FP32 kernel) exactly when d <= 32 and n*K >= 2^20
+    tensor_core = d <= 32 and n * K_ >= 1 << 20
+    assert (launches != launches_fp32) == tensor_core, (launches, launches_fp32)
 
 
 def test_duplicate_codes_resolve_to_the_smallest_index():

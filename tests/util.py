@@ -93,29 +93,7 @@ def _run_ours(view, act, count, dL_dpix, colors_precomp, cov3D_precomp, debug):
     P = means3D.shape[0]
     out.update(num_rendered=R, color=color.cpu().numpy(), radii=radii.cpu().numpy())
     if P > 0:
-        gl, _ = capi.geometry_layout(P)
-        il, _ = capi.image_layout(view.W, view.H)
-        gb, ib, bb = geom.cpu().numpy(), img.cpu().numpy(), binning.cpu().numpy()
-        hdr = np.frombuffer(gb, dtype=np.int32, count=2, offset=0)
-        assert int(hdr[1]) == R, (hdr, R)                 # header[1] = the reference's num_rendered
-        out["num_listed"] = n_listed = int(hdr[0])        # header[0] = instances actually listed (<= R)
-        bl, _ = capi.binning_layout(n_listed, view.W, view.H)
-        N = view.W * view.H
-        tiles = ((view.W + 15) // 16) * ((view.H + 15) // 16)
-
-        def arr(buf, off, dtype, n):
-            return np.frombuffer(buf, dtype=dtype, count=n, offset=off).copy()
-        out["geom"] = dict(
-            depths=arr(gb, gl["depth"], np.float32, P), means2D=arr(gb, gl["means2D"], np.float32, 2 * P).reshape(P, 2),
-            conic_opacity=arr(gb, gl["conic_opacity"], np.float32, 4 * P).reshape(P, 4),
-            rgb=arr(gb, gl["rgb"], np.float32, 4 * P).reshape(P, 4)[:, :3].copy(),
-            cov3D=arr(gb, gl["cov3D"], np.float32, 6 * P).reshape(P, 6), clamped_bits=arr(gb, gl["clamped"], np.uint8, P),
-            tiles_touched=arr(gb, gl["tiles_touched"], np.uint32, P), sorted_ids=arr(gb, gl["sorted_ids"], np.uint32, P),
-            radii=out["radii"])
-        out["final_T"] = arr(ib, il["final_T"], np.float32, N)
-        out["n_contrib"] = arr(ib, il["n_contrib"], np.uint32, N)
-        out["ranges"] = arr(ib, il["ranges"], np.uint32, 2 * tiles).reshape(tiles, 2)
-        out["point_list"] = arr(bb, bl["point_list"], np.uint32, n_listed) if n_listed > 0 else np.zeros(0, np.uint32)
+        out.update(read_state(view, P, R, out["radii"], geom, binning, img))
     if dL_dpix is not None and not count:
         g = _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rots, view.scale_modifier, cov, vm, pm, view.tanfovx,
                                             view.tanfovy, _t(dL_dpix), shs, view.sh_degree, cp, geom, R, binning, img, debug)
@@ -123,6 +101,125 @@ def _run_ours(view, act, count, dL_dpix, colors_precomp, cov3D_precomp, debug):
         out["grads"] = {n: t.cpu().numpy() for n, t in zip(names, g)}
     torch.cuda.synchronize()
     return out
+
+
+def read_state(view: View, P, R, radii, geom, binning, img) -> dict:
+    """The forward state a backward reads, copied out of the three blobs of a forward (plain or fused: same layouts)."""
+    from lightgaussian_b200 import capi
+    gl, _ = capi.geometry_layout(P)
+    il, _ = capi.image_layout(view.W, view.H)
+    gb, ib, bb = geom.cpu().numpy(), img.cpu().numpy(), binning.cpu().numpy()
+    hdr = np.frombuffer(gb, dtype=np.int32, count=2, offset=0)
+    assert int(hdr[1]) == R, (hdr, R)                 # header[1] = the reference's num_rendered
+    n_listed = int(hdr[0])                            # header[0] = instances actually listed (<= R)
+    bl, _ = capi.binning_layout(n_listed, view.W, view.H)
+    N = view.W * view.H
+    tiles = ((view.W + 15) // 16) * ((view.H + 15) // 16)
+
+    def arr(buf, off, dtype, n):
+        return np.frombuffer(buf, dtype=dtype, count=n, offset=off).copy()
+    out = dict(num_listed=n_listed, radii=np.asarray(radii))
+    out["geom"] = dict(
+        depths=arr(gb, gl["depth"], np.float32, P), means2D=arr(gb, gl["means2D"], np.float32, 2 * P).reshape(P, 2),
+        conic_opacity=arr(gb, gl["conic_opacity"], np.float32, 4 * P).reshape(P, 4),
+        rgb=arr(gb, gl["rgb"], np.float32, 4 * P).reshape(P, 4)[:, :3].copy(),
+        cov3D=arr(gb, gl["cov3D"], np.float32, 6 * P).reshape(P, 6), clamped_bits=arr(gb, gl["clamped"], np.uint8, P),
+        tiles_touched=arr(gb, gl["tiles_touched"], np.uint32, P), sorted_ids=arr(gb, gl["sorted_ids"], np.uint32, P),
+        radii=out["radii"])
+    out["final_T"] = arr(ib, il["final_T"], np.float32, N)
+    out["n_contrib"] = arr(ib, il["n_contrib"], np.uint32, N)
+    out["ranges"] = arr(ib, il["ranges"], np.uint32, 2 * tiles).reshape(tiles, 2)
+    out["point_list"] = arr(bb, bl["point_list"], np.uint32, n_listed) if n_listed > 0 else np.zeros(0, np.uint32)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# the float64 oracle's backward on OUR forward state (so no threshold can differ)
+# ------------------------------------------------------------------------------------------------
+def oracle_backward_on_our_state(o, view, act, ours, dpix, colors=None, cov=None):
+    geom = ours["geom"]
+    P = act["means3D"].shape[0]
+    clamped3 = np.stack([(geom["clamped_bits"] >> c) & 1 for c in range(3)], axis=1).astype(np.uint8)
+    col = geom["rgb"] if colors is None else colors
+    g2 = o.blend_backward(view, P, ours["ranges"], ours["point_list"], geom["means2D"], geom["conic_opacity"], col,
+                          ours["final_T"], ours["n_contrib"], dpix)
+    g3 = o.preprocess_backward(view, act["means3D"], ours["radii"], clamped3, geom["cov3D"] if cov is None else cov,
+                               g2["dL_dmean2D"], g2["dL_dconic"], g2["dL_dcolor"],
+                               shs=None if colors is not None else act["shs"],
+                               scales=None if cov is not None else act["scales"],
+                               rotations=None if cov is not None else act["rotations"])
+    return g2, g3
+
+
+LEAVES = ("xyz", "features_dc", "features_rest", "scaling", "rotation", "opacity")
+
+
+def activate(raw: dict, sh_degree: int) -> dict:
+    """The activated inputs the fused kernels compute from GaussianModel's raw leaves (exp / normalize / sigmoid, float32), with the
+    SH rows cut to the (sh_degree+1)^2 coefficients the view uses."""
+    M = (sh_degree + 1) ** 2
+    rot = raw["rotation"].astype(np.float32)
+    n = np.maximum(np.sqrt((rot * rot).sum(1, keepdims=True)), np.float32(1e-12))
+    return dict(means3D=np.ascontiguousarray(raw["xyz"], np.float32), scales=np.exp(raw["scaling"]).astype(np.float32),
+                rotations=(rot / n).astype(np.float32), opacities=(1.0 / (1.0 + np.exp(-raw["opacity"]))).astype(np.float32),
+                shs=np.ascontiguousarray(np.concatenate([raw["features_dc"], raw["features_rest"]], axis=1)[:, :M], np.float32))
+
+
+def leaf_grads_from_activated(raw: dict, g: dict) -> dict:
+    """Chain rule of GaussianModel's activations, in float64: gradients with respect to the activated inputs (keys of
+    Rasterizer::backward: dL_dmeans3D, dL_dsh, dL_dscales, dL_drotations, dL_dopacity, dL_dmeans2D) -> gradients of the six raw
+    leaves and of viewspace_points ("means2D", [P, 3], z column zero)."""
+    P, K = raw["xyz"].shape[0], raw["features_rest"].shape[1]
+    f64 = lambda a: np.asarray(a, np.float64)  # noqa: E731
+    dsh = f64(g["dL_dsh"]).reshape(P, -1, 3)
+    rest = np.zeros((P, K, 3))
+    rest[:, :dsh.shape[1] - 1] = dsh[:, 1:1 + K]
+    v = f64(raw["rotation"])
+    nv = np.maximum(np.sqrt((v * v).sum(1, keepdims=True)), 1e-12)
+    q, gr = v / nv, f64(g["dL_drotations"]).reshape(P, 4)
+    sig = 1.0 / (1.0 + np.exp(-f64(raw["opacity"])))
+    m2 = np.zeros((P, 3))
+    m2[:, :2] = f64(g["dL_dmeans2D"]).reshape(P, -1)[:, :2]
+    return dict(xyz=f64(g["dL_dmeans3D"]).reshape(P, 3), features_dc=dsh[:, :1].copy(), features_rest=rest,
+                scaling=f64(g["dL_dscales"]).reshape(P, 3) * np.exp(f64(raw["scaling"])),
+                rotation=(gr - q * (q * gr).sum(1, keepdims=True)) / nv,
+                opacity=f64(g["dL_dopacity"]).reshape(P, 1) * sig * (1.0 - sig), means2D=m2)
+
+
+def leaf_grads_float64(view: View, raw: dict, state: dict, dpix, act=None) -> dict:
+    """Exact (float64 oracle) gradients of the six raw leaves and of viewspace_points for the upstream gradient `dpix`, evaluated on a
+    given forward state (read_state() of the fused forward), so that every threshold decision is the kernels' own.  `raw` holds the
+    leaves as float32 numpy arrays, features_rest contiguous; view.sh_degree is the active degree.  `act`: the activated inputs the
+    kernels saw (default: activate(raw))."""
+    act = activate(raw, view.sh_degree) if act is None else act
+    g2, g3 = oracle_backward_on_our_state(Oracle(double=True), view, act, state, np.asarray(dpix, np.float32))
+    return leaf_grads_from_activated(raw, dict(dL_dmeans2D=g2["dL_dmean2D"], dL_dopacity=g2["dL_dopacity"], **g3))
+
+
+def element_ratios(ours, exact, rho, alpha):
+    """|ours - exact| / (rho |exact| + alpha max|exact|) per entry (float64); > 1 fails assert_every_element"""
+    a, e = np.asarray(ours, np.float64).ravel(), np.asarray(exact, np.float64).ravel()
+    assert a.shape == e.shape, (a.shape, e.shape)
+    bound = rho * np.abs(e) + alpha * np.abs(e).max(initial=0.0)
+    err = np.abs(a - e)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        r = np.where(err == 0, 0.0, err / bound)
+    return np.where(np.isnan(a), np.inf, r)
+
+
+def assert_every_element(ours, exact, rho, alpha, name):
+    """|ours - exact| <= rho |exact| + alpha max|exact| for EVERY entry (no quantile).  Returns the worst ratio to the bound; on failure
+    the message lists the worst entries."""
+    r = element_ratios(ours, exact, rho, alpha)
+    worst = float(r.max(initial=0.0))
+    if worst > 1.0:
+        a, e = np.asarray(ours, np.float64), np.asarray(exact, np.float64)
+        bad = np.argsort(r)[::-1][:8]
+        rows = [f"  {np.unravel_index(int(i), e.shape)}: ours {a.ravel()[i]:.9g}  exact {e.ravel()[i]:.9g}  ratio {r[i]:.3g}" for i in bad
+                if r[i] > 1.0]
+        raise AssertionError(f"{name}: {int((r > 1.0).sum())} of {r.size} entries outside {rho:g} |exact| + {alpha:g} max|exact| "
+                             f"(max|exact| = {np.abs(e).max(initial=0.0):.3g}); worst:\n" + "\n".join(rows))
+    return worst
 
 
 # ------------------------------------------------------------------------------------------------
