@@ -1,15 +1,9 @@
-"""Import-time stand-in for the simple-knn extension (scene/gaussian_model.py:20 imports it unconditionally;
-it is only *called* when a scene is created from a raw point cloud, which the prune / distill / render
-scripts never do)."""
-import torch
+"""Drop-in for the reference's `simple_knn._C` extension (submodules/simple-knn).  scene/gaussian_model.py:20 imports it at module
+import time, and GaussianModel.create_from_pcd calls distCUDA2 whenever a Scene is built from a dataset's point cloud (every script
+that constructs Scene(dataset, gaussians) without load_iteration).  The native kernel is lightgaussian_b200/csrc/lgr_knn.cuh; importing
+this module loads neither liblgrast.so nor a GPU, the first call does."""
 
 
-def distCUDA2(points: torch.Tensor) -> torch.Tensor:
-    """Mean squared distance to the 3 nearest neighbours, brute force in chunks (init-time only)."""
-    P = points.shape[0]
-    out = torch.empty(P, device=points.device, dtype=points.dtype)
-    step = max(1, min(P, (1 << 26) // max(P, 1)))
-    for s in range(0, P, step):
-        d = torch.cdist(points[s:s + step], points)
-        out[s:s + step] = (d.topk(4, dim=1, largest=False).values[:, 1:] ** 2).mean(dim=1)
-    return out
+def distCUDA2(points):
+    from lightgaussian_b200.knn import distCUDA2 as native
+    return native(points)

@@ -264,6 +264,14 @@ int lgr_vq_gather(int n, int d, const int32_t* idx, const float* embed, float* o
 int lgr_vq_pack_indices(int64_t n, int bits, const int32_t* idx, uint8_t* out, void* cuda_stream);
 int lgr_vq_unpack_indices(int64_t n, int bits, const uint8_t* in, int32_t* idx, void* cuda_stream);
 
+/* ---- initial scales from a point cloud: distCUDA2 of submodules/simple-knn (spatial.cu:15-26, simple_knn.cu:147-221) ----
+ * out[i] = mean of the squared distances from points[i] to its three nearest OTHER points (by index: a duplicate counts, at 0),
+ * bit-identical to the reference's extension on sm_90a (csrc/lgr_knn.cuh).  With fewer than three other points the missing ones
+ * count as FLT_MAX, as in the reference.  points: device [P,3] contiguous float32; out: device [P] float32.
+ * workspace: lgr_knn_workspace_bytes(P) bytes, 256-byte aligned.  No host synchronisation; P == 0 does nothing. */
+size_t lgr_knn_workspace_bytes(int P);
+int lgr_knn_mean_dist3(int P, const float* points, float* out, void* workspace, size_t workspace_bytes, void* cuda_stream);
+
 /* present[i] = (view-space z of point i) > 0.2   (RAST/cuda_rasterizer/rasterizer_impl.cu:54-66, auxiliary.h:139-164) */
 int lgr_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present,
                      void* cuda_stream);

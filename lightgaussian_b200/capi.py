@@ -144,6 +144,10 @@ def load():
         lib.lgr_multimem_allreduce.argtypes = [vp, i32, i32, C.c_size_t, vp]
         lib.lgr_sh_grad_from_views.restype = i32
         lib.lgr_sh_grad_from_views.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+        lib.lgr_knn_workspace_bytes.restype = C.c_size_t
+        lib.lgr_knn_workspace_bytes.argtypes = [i32]
+        lib.lgr_knn_mean_dist3.restype = i32
+        lib.lgr_knn_mean_dist3.argtypes = [i32, vp, vp, vp, C.c_size_t, vp]
         lib.lgr_mark_visible.restype = i32
         lib.lgr_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
         lib.lgr_last_error.restype = C.c_char_p

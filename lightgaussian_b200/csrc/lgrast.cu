@@ -22,6 +22,7 @@
 #include <cub/cub.cuh>
 #include <thrust/iterator/transform_iterator.h>
 #include <thrust/iterator/counting_iterator.h>
+#include <cfloat>
 #include <cmath>
 #include <algorithm>
 #include <atomic>
@@ -1067,6 +1068,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(PreBackArgs a)
 #include "lgr_optim.cuh"
 #include "lgr_vq.cuh"
 #include "lgr_vq_tc.cuh"
+#include "lgr_knn.cuh"
 namespace {
 
 // ------------------------------------------------------------------------------------------------
@@ -2320,6 +2322,51 @@ int lgr_mark_visible(int P, const float* means3D, const float* viewmatrix, const
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     mark_visible_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, means3D, viewmatrix, present);
     LGR_LAUNCH_CHECK("mark_visible_kernel", false, stream);
+    return LGR_OK;
+}
+
+size_t lgr_knn_workspace_bytes(int P) { return knn_layout(P).total; }
+
+int lgr_knn_mean_dist3(int P, const float* points, float* out, void* workspace, size_t workspace_bytes, void* cuda_stream)
+{
+    if (P < 0) {
+        g_last_error = "lgr_knn_mean_dist3: P < 0";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P == 0) return LGR_OK;
+    const KnnLayout L = knn_layout(P);
+    if (!points || !out || !workspace || workspace_bytes < L.total || ((uintptr_t)workspace & 255) || ((uintptr_t)points & 3)) {
+        g_last_error = "lgr_knn_mean_dist3: missing pointer, or workspace smaller than lgr_knn_workspace_bytes(P) / not 256-byte aligned";
+        return LGR_ERR_INVALID_ARG;
+    }
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    char* ws = static_cast<char*>(workspace);
+    unsigned* bbox = reinterpret_cast<unsigned*>(ws + L.bbox);
+    uint32_t* codes = reinterpret_cast<uint32_t*>(ws + L.codes);
+    uint32_t* codes_sorted = reinterpret_cast<uint32_t*>(ws + L.codes_sorted);
+    uint32_t* ids = reinterpret_cast<uint32_t*>(ws + L.ids);
+    uint32_t* ids_sorted = reinterpret_cast<uint32_t*>(ws + L.ids_sorted);
+    float4* sorted = reinterpret_cast<float4*>(ws + L.sorted);
+    float4* leafbox = reinterpret_cast<float4*>(ws + L.leafbox);
+    float4* nodebox = reinterpret_cast<float4*>(ws + L.nodebox);
+    const int nleaf = (P + KNN_LEAF - 1) / KNN_LEAF, nnode = (nleaf + KNN_NODE - 1) / KNN_NODE;
+
+    LGR_CUDA_TRY(cudaMemsetAsync(bbox, 0xff, 3 * sizeof(unsigned), stream));
+    LGR_CUDA_TRY(cudaMemsetAsync(bbox + 3, 0, 3 * sizeof(unsigned), stream));
+    knn_bbox_kernel<<<std::min((P + 255) / 256, 4 * LGR_SMS), 256, 0, stream>>>(P, points, bbox);
+    LGR_LAUNCH_CHECK("knn_bbox_kernel", false, stream);
+    knn_morton_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, points, bbox, codes, ids);
+    LGR_LAUNCH_CHECK("knn_morton_kernel", false, stream);
+    size_t cub_bytes = L.cub_bytes;
+    LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(ws + L.cub, cub_bytes, codes, codes_sorted, ids, ids_sorted, P, 0, 30, stream));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    knn_leaf_kernel<<<(nleaf + 7) / 8, 256, 0, stream>>>(P, nleaf, points, ids_sorted, sorted, leafbox);
+    LGR_LAUNCH_CHECK("knn_leaf_kernel", false, stream);
+    knn_node_kernel<<<(nnode + 7) / 8, 256, 0, stream>>>(nleaf, nnode, leafbox, nodebox);
+    LGR_LAUNCH_CHECK("knn_node_kernel", false, stream);
+    constexpr int warps = KNN_SEARCH_THREADS / 32;
+    knn_search_kernel<<<(nleaf + warps - 1) / warps, KNN_SEARCH_THREADS, 0, stream>>>(P, nleaf, nnode, sorted, leafbox, nodebox, out);
+    LGR_LAUNCH_CHECK("knn_search_kernel", false, stream);
     return LGR_OK;
 }
 
