@@ -272,6 +272,43 @@ int lgr_vq_unpack_indices(int64_t n, int bits, const uint8_t* in, int32_t* idx, 
 size_t lgr_knn_workspace_bytes(int P);
 int lgr_knn_mean_dist3(int P, const float* points, float* out, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
+/* ---- densification: GaussianModel.add_densification_stats / densify_and_prune (scene/gaussian_model.py:602-788) ----
+ * Bit-identical to the reference's torch code (csrc/lgr_densify.cuh).  All pointers are device pointers to contiguous float32.
+ * lgr_densify_stats: for rows with update_filter[i] != 0, accum[i] += |grad[i, 0:2]| and denom[i] += 1; grad rows are
+ *   grad_row_stride floats apart.  No host synchronisation.
+ * lgr_densify_plan: classifies every row (clone, split, prune) from accum, denom, the raw scaling [P,3] and the raw opacity [P].
+ *   Thresholds are float32, as torch compares a float tensor with a Python scalar: max_grad, dense_scale = percent_dense*extent,
+ *   min_opacity, big_scale = 0.1*extent.  prune_all removes every row (the reference's big_points_vs on its just-zeroed radii, when
+ *   0 > max_screen_size); prune_big enables the big_scale test.  Returns counts_host[4] = {kept original rows, kept clones, kept
+ *   split children per copy, split rows S} after one stream synchronisation.  workspace: lgr_densify_workspace_bytes(P) bytes,
+ *   256-byte aligned; lgr_densify_rows reads it, so it must stay untouched in between.
+ * lgr_densify_split_inputs: the operands of the split's product bmm(build_rotation(q), samples) for the 2S children, rows r and
+ *   S + r for the split row of rank r, as the reference's .repeat(2, 1) lays them out: rotations_out [2S,3,3] and samples_out [2S,3] =
+ *   normals * exp(scaling) + 0.  normals: [2S,3] standard normals drawn by the caller through torch's generator.  No fixed operation
+ *   order of that 3x3 . 3x1 product matches torch.bmm on every sample, so the caller forms it with torch.bmm.
+ * lgr_densify_rows: writes the rows_out = counts[0] + counts[1] + 2*counts[2] output rows of up to 24 tensors in one launch, in the
+ *   order unsplit rows, clones, first children, second children.  child_offsets: [2S,3] product of lgr_densify_split_inputs' operands,
+ *   added to the parents' xyz.  Roles: COPY = raw copy to every destination; XYZ / SCALING = copied, computed for the children
+ *   (row_words 3); MOMENT = copied to the kept original row, zero for new rows; ZERO = zero everywhere (src may be NULL).  Tensors
+ *   with row_words == 0 are skipped, their pointers are not read. */
+enum { LGR_DENSIFY_COPY = 0, LGR_DENSIFY_XYZ = 1, LGR_DENSIFY_SCALING = 2, LGR_DENSIFY_MOMENT = 3, LGR_DENSIFY_ZERO = 4 };
+typedef struct lgr_densify_tensor {
+    const void* src;
+    void* dst;
+    int32_t row_words;
+    int32_t role;
+} lgr_densify_tensor;
+int lgr_densify_stats(int P, const float* grad, int grad_row_stride, const uint8_t* update_filter, float* accum, float* denom,
+                      void* cuda_stream);
+size_t lgr_densify_workspace_bytes(int P);
+int lgr_densify_plan(int P, const float* accum, const float* denom, const float* scaling, const float* opacity, float max_grad,
+                     float dense_scale, float min_opacity, float big_scale, int prune_all, int prune_big, void* workspace,
+                     size_t workspace_bytes, int32_t* counts_host, void* cuda_stream);
+int lgr_densify_split_inputs(int P, const void* workspace, const int32_t* counts, const float* scaling, const float* rotation,
+                             const float* normals, float* rotations_out, float* samples_out, void* cuda_stream);
+int lgr_densify_rows(int P, const void* workspace, const int32_t* counts, const float* xyz, const float* child_offsets, int n_tensors,
+                     const lgr_densify_tensor* tensors, void* cuda_stream);
+
 /* present[i] = (view-space z of point i) > 0.2   (RAST/cuda_rasterizer/rasterizer_impl.cu:54-66, auxiliary.h:139-164) */
 int lgr_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present,
                      void* cuda_stream);

@@ -53,6 +53,14 @@ class LgrCompactTensor(C.Structure):
     _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("row_words", C.c_int32)]
 
 
+class LgrDensifyTensor(C.Structure):
+    """struct lgr_densify_tensor"""
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("row_words", C.c_int32), ("role", C.c_int32)]
+
+
+DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING, DENSIFY_MOMENT, DENSIFY_ZERO = range(5)   # LGR_DENSIFY_* roles
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 
 _lib = None
@@ -148,6 +156,17 @@ def load():
         lib.lgr_knn_workspace_bytes.argtypes = [i32]
         lib.lgr_knn_mean_dist3.restype = i32
         lib.lgr_knn_mean_dist3.argtypes = [i32, vp, vp, vp, C.c_size_t, vp]
+        lib.lgr_densify_stats.restype = i32
+        lib.lgr_densify_stats.argtypes = [i32, vp, i32, vp, vp, vp, vp]
+        lib.lgr_densify_workspace_bytes.restype = C.c_size_t
+        lib.lgr_densify_workspace_bytes.argtypes = [i32]
+        lib.lgr_densify_plan.restype = i32
+        lib.lgr_densify_plan.argtypes = [i32, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float, C.c_float, i32, i32, vp, C.c_size_t,
+                                         C.POINTER(C.c_int32), vp]
+        lib.lgr_densify_split_inputs.restype = i32
+        lib.lgr_densify_split_inputs.argtypes = [i32, vp, C.POINTER(C.c_int32), vp, vp, vp, vp, vp, vp]
+        lib.lgr_densify_rows.restype = i32
+        lib.lgr_densify_rows.argtypes = [i32, vp, C.POINTER(C.c_int32), vp, vp, i32, C.POINTER(LgrDensifyTensor), vp]
         lib.lgr_mark_visible.restype = i32
         lib.lgr_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
         lib.lgr_last_error.restype = C.c_char_p

@@ -1069,6 +1069,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(PreBackArgs a)
 #include "lgr_vq.cuh"
 #include "lgr_vq_tc.cuh"
 #include "lgr_knn.cuh"
+#include "lgr_densify.cuh"
 namespace {
 
 // ------------------------------------------------------------------------------------------------
@@ -2367,6 +2368,143 @@ int lgr_knn_mean_dist3(int P, const float* points, float* out, void* workspace, 
     constexpr int warps = KNN_SEARCH_THREADS / 32;
     knn_search_kernel<<<(nleaf + warps - 1) / warps, KNN_SEARCH_THREADS, 0, stream>>>(P, nleaf, nnode, sorted, leafbox, nodebox, out);
     LGR_LAUNCH_CHECK("knn_search_kernel", false, stream);
+    return LGR_OK;
+}
+
+}  // extern "C"
+
+// ---- densification (csrc/lgr_densify.cuh) ----
+namespace {
+struct DensifyLayout {
+    size_t cls, scan, counts, cub, cub_bytes, total;
+};
+DensifyLayout densify_layout(int P)
+{
+    DensifyLayout L{};
+    const int n = P > 0 ? P : 1;
+    L.cls = 0;
+    L.scan = align_up((size_t)n, 256);
+    L.counts = align_up(L.scan + sizeof(int4) * (size_t)n, 256);
+    L.cub = L.counts + 256;
+    cub::DeviceScan::InclusiveScan((void*)nullptr, L.cub_bytes, thrust::make_transform_iterator((const uint8_t*)nullptr, DenClassCounts()),
+                                   (int4*)nullptr, DenInt4Sum(), n);
+    L.total = align_up(L.cub + L.cub_bytes, 256);
+    return L;
+}
+}  // namespace
+
+extern "C" {
+
+int lgr_densify_stats(int P, const float* grad, int grad_row_stride, const uint8_t* update_filter, float* accum, float* denom,
+                      void* cuda_stream)
+{
+    if (P < 0 || grad_row_stride < 2 || (P && (!grad || !update_filter || !accum || !denom))) {
+        g_last_error = "lgr_densify_stats: bad argument (P >= 0, grad_row_stride >= 2, all pointers set)";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P == 0) return LGR_OK;
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    densify_stats_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, grad, grad_row_stride, update_filter, accum, denom);
+    LGR_LAUNCH_CHECK("densify_stats_kernel", false, stream);
+    return LGR_OK;
+}
+
+size_t lgr_densify_workspace_bytes(int P) { return densify_layout(P).total; }
+
+int lgr_densify_plan(int P, const float* accum, const float* denom, const float* scaling, const float* opacity, float max_grad,
+                     float dense_scale, float min_opacity, float big_scale, int prune_all, int prune_big, void* workspace,
+                     size_t workspace_bytes, int32_t* counts_host, void* cuda_stream)
+{
+    if (P < 0 || !counts_host) {
+        g_last_error = "lgr_densify_plan: bad argument";
+        return LGR_ERR_INVALID_ARG;
+    }
+    for (int k = 0; k < 4; k++) counts_host[k] = 0;
+    if (P == 0) return LGR_OK;
+    const DensifyLayout L = densify_layout(P);
+    if (!accum || !denom || !scaling || !opacity || !workspace || workspace_bytes < L.total || ((uintptr_t)workspace & 255)) {
+        g_last_error = "lgr_densify_plan: missing pointer, or workspace smaller than lgr_densify_workspace_bytes(P) / not 256-byte aligned";
+        return LGR_ERR_INVALID_ARG;
+    }
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    char* ws = static_cast<char*>(workspace);
+    uint8_t* cls = reinterpret_cast<uint8_t*>(ws + L.cls);
+    int4* scan = reinterpret_cast<int4*>(ws + L.scan);
+    const DensifyPlanArgs a{accum, denom, scaling, opacity, max_grad, dense_scale, min_opacity, big_scale, prune_all ? 1 : 0, prune_big ? 1 : 0};
+    densify_plan_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, a, cls);
+    LGR_LAUNCH_CHECK("densify_plan_kernel", false, stream);
+    size_t cub_bytes = L.cub_bytes;
+    LGR_CUDA_TRY(cub::DeviceScan::InclusiveScan(ws + L.cub, cub_bytes, thrust::make_transform_iterator((const uint8_t*)cls, DenClassCounts()),
+                                                scan, DenInt4Sum(), P, stream));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    LGR_CUDA_TRY(cudaMemcpyAsync(counts_host, scan + (P - 1), sizeof(int4), cudaMemcpyDeviceToHost, stream));
+    LGR_CUDA_TRY(cudaStreamSynchronize(stream));
+    return LGR_OK;
+}
+
+int lgr_densify_split_inputs(int P, const void* workspace, const int32_t* counts, const float* scaling, const float* rotation,
+                             const float* normals, float* rotations_out, float* samples_out, void* cuda_stream)
+{
+    if (P < 0 || !counts) {
+        g_last_error = "lgr_densify_split_inputs: bad argument";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P == 0 || counts[3] == 0) return LGR_OK;
+    if (!workspace || ((uintptr_t)workspace & 255) || !scaling || !rotation || ((uintptr_t)rotation & 15) || !normals || !rotations_out ||
+        !samples_out) {
+        g_last_error = "lgr_densify_split_inputs: missing pointer, or a workspace / rotation pointer that is not aligned";
+        return LGR_ERR_INVALID_ARG;
+    }
+    const char* ws = static_cast<const char*>(workspace);
+    const DensifyLayout L = densify_layout(P);
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    densify_split_inputs_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, reinterpret_cast<const uint8_t*>(ws + L.cls),
+                                                                     reinterpret_cast<const int4*>(ws + L.scan), scaling, rotation, normals,
+                                                                     counts[3], rotations_out, samples_out);
+    LGR_LAUNCH_CHECK("densify_split_inputs_kernel", false, stream);
+    return LGR_OK;
+}
+
+int lgr_densify_rows(int P, const void* workspace, const int32_t* counts, const float* xyz, const float* child_offsets, int n_tensors,
+                     const lgr_densify_tensor* tensors, void* cuda_stream)
+{
+    if (P < 0 || !counts || n_tensors < 0 || n_tensors > DEN_MAX_TENSORS || (n_tensors && !tensors)) {
+        g_last_error = "lgr_densify_rows: bad argument (at most 24 tensors per call)";
+        return LGR_ERR_INVALID_ARG;
+    }
+    const long long rows_out = (long long)counts[0] + counts[1] + 2LL * counts[2];
+    if (P == 0 || rows_out == 0 || n_tensors == 0) return LGR_OK;
+    if (!workspace || ((uintptr_t)workspace & 255) || !xyz || (counts[2] && !child_offsets)) {
+        g_last_error = "lgr_densify_rows: missing pointer, or a workspace that is not 256-byte aligned";
+        return LGR_ERR_INVALID_ARG;
+    }
+    DensifyTable t;
+    memset(&t, 0, sizeof(t));
+    for (int i = 0; i < n_tensors; i++) {
+        const lgr_densify_tensor& d = tensors[i];
+        const bool geometric = d.role == LGR_DENSIFY_XYZ || d.role == LGR_DENSIFY_SCALING;
+        if (d.role < LGR_DENSIFY_COPY || d.role > LGR_DENSIFY_ZERO || d.row_words < 0 || (geometric && d.row_words != 3)) {
+            g_last_error = "lgr_densify_rows: tensor with a bad role or a bad row width";
+            return LGR_ERR_INVALID_ARG;
+        }
+        if (d.row_words == 0) continue;   // an empty row, such as _features_rest [P,0,3] at SH degree 0: nothing to write
+        if (!d.dst || (!d.src && d.role != LGR_DENSIFY_ZERO)) {
+            g_last_error = "lgr_densify_rows: tensor with a missing pointer";
+            return LGR_ERR_INVALID_ARG;
+        }
+        t.src[t.count] = static_cast<const float*>(d.src);
+        t.dst[t.count] = static_cast<float*>(d.dst);
+        t.width[t.count] = d.row_words;
+        t.role[t.count] = d.role;
+        t.count++;
+    }
+    const char* ws = static_cast<const char*>(workspace);
+    const DensifyLayout L = densify_layout(P);
+    const DensifyRowsArgs a{reinterpret_cast<const uint8_t*>(ws + L.cls), reinterpret_cast<const int4*>(ws + L.scan), xyz, child_offsets,
+                            counts[0], counts[1], counts[2], counts[3]};
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    densify_rows_kernel<<<(unsigned)((P + 7) / 8), 256, 0, stream>>>(P, t, a);
+    LGR_LAUNCH_CHECK("densify_rows_kernel", false, stream);
     return LGR_OK;
 }
 

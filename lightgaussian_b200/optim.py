@@ -53,7 +53,8 @@ class FusedAdamW(torch.optim.AdamW):
                 # the distillation student's _features_rest[:, :8, :] (scene/gaussian_model.py:129-136; registered as is by
                 # distill_train.py:79) through (row_elems, row_stride); the keys of optimizer.state stay the caller's tensors
                 row_elems = row_stride = 0
-                if not p.is_contiguous():
+                permuted = not p.is_contiguous() and _permuted_dense(p)
+                if not p.is_contiguous() and not permuted:
                     trace.bump("adamw_strided_params")
                     row_elems, row_stride = _row_strided(p)
                     if row_elems == 0:
@@ -65,10 +66,17 @@ class FusedAdamW(torch.optim.AdamW):
                     state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)      # dense for a non-dense view
                     state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                 state["step"] += 1
-                g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
                 m, v = state["exp_avg"], state["exp_avg_sq"]
-                if not (m.is_contiguous() and v.is_contiguous()):
-                    raise RuntimeError("FusedAdamW: optimizer state must be contiguous")
+                if permuted:
+                    # a dense parameter in a permuted layout, such as the _xyz GaussianModel.create_from_pcd builds from a transposed numpy
+                    # array: the update is element-wise, so every tensor is walked in the parameter's own memory order
+                    g = p.grad if p.grad.stride() == p.stride() else torch.empty_like(p).copy_(p.grad)
+                    if m.stride() != p.stride() or v.stride() != p.stride():
+                        raise RuntimeError("FusedAdamW: optimizer state must have its parameter's layout")
+                else:
+                    g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
+                    if not (m.is_contiguous() and v.is_contiguous()):
+                        raise RuntimeError("FusedAdamW: optimizer state must be contiguous")
                 key = (p.device, float(beta1), float(beta2), float(group["eps"]), float(group["weight_decay"]))
                 by_cfg.setdefault(key, []).append((p, g, m, v, float(group["lr"]), float(state["step"]), row_elems, row_stride))
         for (device, beta1, beta2, eps, wd), items in by_cfg.items():
@@ -83,6 +91,16 @@ class FusedAdamW(torch.optim.AdamW):
                     st = lib.lgr_adamw_step(len(chunk), arr, beta1, beta2, eps, wd, capi.current_stream_ptr(device))
                 capi.check(st, "lgr_adamw_step")
         return loss
+
+
+def _permuted_dense(p):
+    """True when `p` fills its memory exactly once in some order of its dimensions (a transposed or permuted dense tensor)"""
+    expect = 1
+    for d in sorted(range(p.dim()), key=p.stride):
+        if p.size(d) != 1 and p.stride(d) != expect:
+            return False
+        expect *= p.size(d)
+    return True
 
 
 def _row_strided(p):
@@ -188,7 +206,8 @@ def to_fused(optimizer):
 def install(GaussianModel):
     """Make a GaussianModel class (scene/gaussian_model.py) use the fused optimizer step and prune compaction without editing it:
     `training_setup` (:176-224) is wrapped so that the AdamW it builds is replaced by an equivalent FusedAdamW, and `prune_points`
-    (:587-600) becomes `optim.prune_points`.  Idempotent."""
+    (:587-600) becomes `optim.prune_points`.  When the class defines `add_densification_stats` and `densify_and_prune` (:745-788),
+    they become the native ones of `densify`.  Idempotent."""
     if getattr(GaussianModel, "_lgr_fused_optim", False):
         return GaussianModel
     original_setup = GaussianModel.training_setup
@@ -201,5 +220,8 @@ def install(GaussianModel):
     training_setup.__wrapped__ = original_setup
     GaussianModel.training_setup = training_setup
     GaussianModel.prune_points = prune_points
+    if hasattr(GaussianModel, "add_densification_stats") and hasattr(GaussianModel, "densify_and_prune"):
+        from . import densify
+        densify.install(GaussianModel)
     GaussianModel._lgr_fused_optim = True
     return GaussianModel
