@@ -14,5 +14,10 @@ if GaussianModel is not None and _os.environ.get("LGR_FUSED_OPTIM", "1") != "0":
     # and prune_points uses the fused compaction; LGR_FUSED_OPTIM=0 keeps torch.optim.AdamW and the reference's surgery.
     from lightgaussian_b200 import optim as _optim
     _optim.install(GaussianModel)
+if GaussianModel is not None and hasattr(GaussianModel, "load_vq") and _os.environ.get("LGR_FUSED", "1") != "0":
+    # render.py / render_video.py --load_vq: the compressed model stays resident and render() reads it in place; the five leaves
+    # other than _xyz are built only when something reads or assigns one.  LGR_FUSED=0 keeps the reference's dense load_vq.
+    from lightgaussian_b200 import vqresident as _vqresident
+    _vqresident.install(GaussianModel)
 if GaussianModel is None:
     del GaussianModel

@@ -134,6 +134,33 @@ int lgr_forward_raw(const lgr_view* view, int P, int M, const lgr_raw_params* pa
                     float* out_color, int32_t* gaussians_count, float* important_score, int32_t* radii,
                     int32_t* num_rendered, void* cuda_stream);
 
+/* ---- rendering a VecTree-compressed model in place (render.py / render_video.py --load_vq) ----
+ * The arrays of extreme_saving/ (vectree/vectree.py:107-155) as they stay resident on the GPU; no [P,dim] table is built.  The
+ * forward reads them instead of the six float32 leaves GaussianModel.load_vq (scene/gaussian_model.py:420-461) would inflate them
+ * to, with the same activations, so the image, radii and significance outputs are bit-identical to lgr_forward_raw on those leaves.
+ * All arrays are device memory, 16-byte aligned. */
+typedef struct lgr_vq_resident_params {
+    const float* xyz;      /* [P,3] float32 */
+    const void* attr;      /* [P,8] raw opacity | scale x3 | rotation x4 (other_attribute.npz order): fp16 if attr_half, else float32 */
+    const int32_t* slot;   /* [P]: >= 0 a codebook row; < 0 the row -(slot) - 1 of nonvq */
+    const void* codebook;  /* [K,Dp] fp16 */
+    const void* nonvq;     /* [Pn,Dp] fp16 if nonvq_half, else float32; may be NULL when no slot is negative */
+    int32_t attr_half;
+    int32_t nonvq_half;
+    int32_t D;  /* colour values per row, 3*(max_degree+1)^2: f_dc_0..2, then f_rest channel-major (row[3 + c*(M-1) + j]) */
+    int32_t Dp; /* row pitch of codebook and nonvq in elements: a multiple of 8, >= D */
+    int32_t K;  /* codebook rows */
+} lgr_vq_resident_params;
+
+/* Forward of a resident VQ model: the allocator, output and stream contract of lgr_forward_raw (M = D/3).  gaussians_count /
+ * important_score are both NULL or both set.  There is no backward: a model that is trained gets its leaves materialised. */
+int lgr_forward_vq(const lgr_view* view, int P, const lgr_vq_resident_params* params,
+                   lgr_alloc_fn geometry_alloc, void* geometry_user,
+                   lgr_alloc_fn binning_alloc, void* binning_user,
+                   lgr_alloc_fn image_alloc, void* image_user,
+                   float* out_color, int32_t* gaussians_count, float* important_score, int32_t* radii,
+                   int32_t* num_rendered, void* cuda_stream);
+
 int lgr_backward_raw(const lgr_view* view, int P, int M, int num_rendered, const lgr_raw_params* params,
                      const int32_t* radii, char* geometry_blob, char* binning_blob, char* image_blob,
                      const float* dL_dout_color, const lgr_raw_grads* grads, float* dL_dmeans2D, void* cuda_stream);

@@ -42,6 +42,12 @@ class LgrRawGrads(C.Structure):
     _fields_ = _SIX_LEAVES + [("rgb", C.c_void_p)]
 
 
+class LgrVqResidentParams(C.Structure):
+    """struct lgr_vq_resident_params: the resident arrays of a VecTree-compressed model"""
+    _fields_ = [("xyz", C.c_void_p), ("attr", C.c_void_p), ("slot", C.c_void_p), ("codebook", C.c_void_p), ("nonvq", C.c_void_p),
+                ("attr_half", C.c_int32), ("nonvq_half", C.c_int32), ("D", C.c_int32), ("Dp", C.c_int32), ("K", C.c_int32)]
+
+
 class LgrAdamwTensor(C.Structure):
     """struct lgr_adamw_tensor"""
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
@@ -98,6 +104,9 @@ def load():
         lib.lgr_forward_raw.restype = i32
         lib.lgr_forward_raw.argtypes = [C.POINTER(LgrView), i32, i32, C.POINTER(LgrRawParams), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp,
                                         vp, vp, vp, vp, C.POINTER(C.c_int32), vp]
+        lib.lgr_forward_vq.restype = i32
+        lib.lgr_forward_vq.argtypes = [C.POINTER(LgrView), i32, C.POINTER(LgrVqResidentParams), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp,
+                                       vp, vp, vp, vp, C.POINTER(C.c_int32), vp]
         lib.lgr_backward_raw.restype = i32
         lib.lgr_backward_raw.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
                                          C.POINTER(LgrRawGrads), vp, vp]

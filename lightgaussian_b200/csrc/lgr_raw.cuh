@@ -74,16 +74,11 @@ struct RawArgs {
     int P, D, M, W, H, gx, gy;
     float fx, fy, tanx, tany, mod;
     const float* xyz;
-    const float* dc;
-    const float* rest;
-    const float* scaling;
-    const float* rotation;
-    const float* opacity;
     const float* view;
     const float* proj;
     const float* campos;
     int prefiltered;
-    int rest_stride;  // floats between consecutive rows of `rest` (>= (M-1)*3; equal when the leaf is dense)
+    int rest_stride;  // floats per staged features_rest row (>= (M-1)*3; equal when the rows are dense)
 };
 
 // dynamic shared memory: 8 warp slices [32*stride floats rest | 32*3 floats dc], then 8 mbarriers, then camera (36 floats).
@@ -112,7 +107,103 @@ __device__ __forceinline__ bool warp_stage_sh_begin(const float* __restrict__ re
     return bulk;
 }
 
-__global__ void __launch_bounds__(256) preprocess_raw_kernel(RawArgs a, int* __restrict__ radii, GeometryState g)
+// ---- attribute and colour sources of preprocess_raw_kernel ----
+// A source hands the kernel the RAW (pre-activation) scaling, rotation and opacity of Gaussian i and stages a warp's SH rows into
+// shared memory as float32 in the leaves' layout (per lane: rest [(M-1)][3] at `nrest` floats per lane, dc [3]).  Everything else
+// -- projection, activations, tile-keep mask, sh_to_rgb -- is the one kernel body, so every source renders bit-identically to the
+// float32 leaves holding the same values.
+
+// GaussianModel's six float32 leaves (scene/gaussian_model.py:46-56); features_rest rows may be row-strided (RawArgs::rest_stride).
+struct LeafSource {
+    const float* dc;
+    const float* rest;
+    const float* scaling_;
+    const float* rotation_;
+    const float* opacity_;
+    __device__ __forceinline__ float scaling(int i, int k) const { return scaling_[3 * (size_t)i + k]; }
+    __device__ __forceinline__ float4 rotation(int i) const { return reinterpret_cast<const float4*>(rotation_)[i]; }
+    __device__ __forceinline__ float opacity(int i) const { return opacity_[i]; }
+    __device__ __forceinline__ bool stage(int nrest, int first, int n, unsigned, float* s_rest, float* s_dc, uint64_t* bar, int lane) const
+    {
+        return warp_stage_sh_begin(rest, dc, nrest, first, n, s_rest, s_dc, bar, lane);
+    }
+};
+
+// A VecTree-compressed model as extreme_saving/ stores it (lgr_vq_resident_params): attributes [P,8] = opacity | scale x3 | rot x4 in
+// fp16 or float32, and per Gaussian either a codebook row (slot >= 0) or its own row of `nonvq` (slot = -(row) - 1).  Colour rows
+// hold D = 3M values in PLY order, f_dc_0..2 then f_rest CHANNEL-major (row[3 + c*(M-1) + j]), `Dp` elements apart; staging
+// transposes them to the leaves' coefficient-major layout.  fp16 -> float32 is exact, so the staged values are those of the
+// float32 leaves GaussianModel.load_vq builds from the same files.
+struct VqSource {
+    const void* attr;
+    const int* slot;
+    const __half* codebook;
+    const void* nonvq;
+    int attr_half, nonvq_half, D, Dp, M;
+    __device__ __forceinline__ float attr_at(int i, int k) const
+    {
+        return attr_half ? __half2float(static_cast<const __half*>(attr)[8 * (size_t)i + k]) : static_cast<const float*>(attr)[8 * (size_t)i + k];
+    }
+    __device__ __forceinline__ float scaling(int i, int k) const { return attr_at(i, 1 + k); }
+    __device__ __forceinline__ float opacity(int i) const { return attr_at(i, 0); }
+    __device__ __forceinline__ float4 rotation(int i) const
+    {
+        if (!attr_half) return reinterpret_cast<const float4*>(attr)[2 * (size_t)i + 1];
+        const uint2 u = reinterpret_cast<const uint2*>(attr)[2 * (size_t)i + 1];
+        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+        return make_float4(a.x, a.y, b.x, b.y);
+    }
+    // The warp's visible rows are fetched in 16-byte pieces spread over all lanes: consecutive non-VQ rows (slots are a prefix
+    // count) are read coalesced, codebook rows are gathers from an L2-resident table.  Plain stores: the caller's __syncwarp orders them.
+    __device__ __forceinline__ bool stage(int nrest, int first, int n, unsigned vis, float* s_rest, float* s_dc, uint64_t*, int lane) const
+    {
+        const int per_row = nonvq_half ? Dp / 8 : Dp / 4;  // 16-byte pieces of the widest row
+        const int total = n * per_row;
+        const int my_slot = lane < n ? slot[first + lane] : 0;  // one coalesced load; pieces get their row's slot by shuffle
+        for (int base = 0; base < total; base += 32) {      // warp-uniform trip count: every lane takes part in the shuffle
+            const int c = base + lane;
+            const int g = min(c, total - 1) / per_row, part = c - g * per_row;
+            const int s = __shfl_sync(0xffffffffu, my_slot, g);
+            if (c >= total || !((vis >> g) & 1u)) continue;
+            float v[8];
+            int e0, cnt;
+            if (s >= 0 || nonvq_half) {
+                if (part * 8 >= Dp) continue;
+                const __half* row = s >= 0 ? codebook + (size_t)s * Dp : static_cast<const __half*>(nonvq) + (size_t)(-s - 1) * Dp;
+                const uint4 u = *reinterpret_cast<const uint4*>(row + part * 8);
+                const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const float2 f = __half22float2(h[k]);
+                    v[2 * k] = f.x;
+                    v[2 * k + 1] = f.y;
+                }
+                e0 = part * 8;
+                cnt = 8;
+            } else {
+                const float4 f = reinterpret_cast<const float4*>(static_cast<const float*>(nonvq) + (size_t)(-s - 1) * Dp)[part];
+                v[0] = f.x; v[1] = f.y; v[2] = f.z; v[3] = f.w;
+                e0 = part * 4;
+                cnt = 4;
+            }
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const int e = e0 + k;
+                if (k >= cnt) break;
+                if (e < 3) {
+                    s_dc[3 * g + e] = v[k];
+                } else if (e < D) {
+                    const int ch = (e - 3) / (M - 1), j = (e - 3) - ch * (M - 1);
+                    s_rest[g * nrest + 3 * j + ch] = v[k];
+                }
+            }
+        }
+        return false;
+    }
+};
+
+template <class Src>
+__global__ void __launch_bounds__(256) preprocess_raw_kernel(RawArgs a, Src src, int* __restrict__ radii, GeometryState g)
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
     const int nrest = a.rest_stride;   // floats per staged row (the leaf's row stride)
@@ -146,9 +237,9 @@ __global__ void __launch_bounds__(256) preprocess_raw_kernel(RawArgs a, int* __r
         x = a.xyz[3 * (size_t)i]; y = a.xyz[3 * (size_t)i + 1]; z = a.xyz[3 * (size_t)i + 2];
         visible = lgr::xform_row(view, 2, x, y, z) > 0.2f;
         if (visible) {
-            const float s0 = act_exp(a.scaling[3 * (size_t)i]), s1 = act_exp(a.scaling[3 * (size_t)i + 1]), s2 = act_exp(a.scaling[3 * (size_t)i + 2]);
+            const float s0 = act_exp(src.scaling(i, 0)), s1 = act_exp(src.scaling(i, 1)), s2 = act_exp(src.scaling(i, 2));
             float dn;
-            const float4 q = act_normalize(reinterpret_cast<const float4*>(a.rotation)[i], dn);
+            const float4 q = act_normalize(src.rotation(i), dn);
             lgr::cov3d_from_scale_rot(s0, s1, s2, a.mod, q.x, q.y, q.z, q.w, cov);
 #pragma unroll
             for (int k = 0; k < 6; k++) g.cov3D[6 * (size_t)i + k] = cov[k];
@@ -158,12 +249,13 @@ __global__ void __launch_bounds__(256) preprocess_raw_kernel(RawArgs a, int* __r
             __trap();
         }
     }
-    const bool any_vis = __any_sync(FULL, visible);
+    const unsigned vis_bits = __ballot_sync(FULL, visible);
+    const bool any_vis = vis_bits != 0u;
     bool bulk = false;
-    if (any_vis) bulk = warp_stage_sh_begin(a.rest, a.dc, nrest, first, n, s_rest, s_dc, &bars[warp], lane);
+    if (any_vis) bulk = src.stage(nrest, first, n, vis_bits, s_rest, s_dc, &bars[warp], lane);
 
     // everything that does not need the SH rows overlaps the copy
-    const float op_act = visible ? act_sigmoid(a.opacity[i]) : 0.f;
+    const float op_act = visible ? act_sigmoid(src.opacity(i)) : 0.f;
     const unsigned long long keep_bits = warp_tile_keep_mask(visible, geo, make_float4(geo.conic_x, geo.conic_y, geo.conic_z, op_act), a.W, a.H, lane);
     if (valid) {
         if (!g.bin_rec) g.iota[i] = (uint32_t)i;

@@ -19,6 +19,7 @@
 //                               (warp, Gaussian) instead of 9 per (pixel, Gaussian)              (K6)
 //   preprocess_backward_kernel  conic/mean2D/colour gradients -> all dense per-Gaussian outputs  (K7+K8 fused)
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
 #include <cub/cub.cuh>
 #include <thrust/iterator/transform_iterator.h>
 #include <thrust/iterator/counting_iterator.h>
@@ -1114,13 +1115,32 @@ __global__ void set_capacity_kernel(int* header, int capacity)
     }
 }
 
+// the geometry fields of the raw-leaf / resident preprocess, from the plain preprocess arguments
+inline RawArgs raw_args(const PreprocessArgs& a, int gx, int gy)
+{
+    RawArgs ra;
+    ra.P = a.P; ra.D = a.D; ra.M = a.M; ra.W = a.W; ra.H = a.H; ra.gx = gx; ra.gy = gy;
+    ra.fx = a.fx; ra.fy = a.fy; ra.tanx = a.tanx; ra.tany = a.tany; ra.mod = a.mod;
+    ra.xyz = nullptr; ra.view = a.view; ra.proj = a.proj; ra.campos = a.campos;
+    ra.prefiltered = a.prefiltered;
+    ra.rest_stride = 0;
+    return ra;
+}
+
 int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const float* shs, const float* colors_precomp,
                  const float* opacities, const float* scales, const float* rotations, const float* cov3D_precomp,
                  lgr_alloc_fn geometry_alloc, void* geometry_user, lgr_alloc_fn binning_alloc, void* binning_user,
                  lgr_alloc_fn image_alloc, void* image_user, float* out_color, int32_t* gaussians_count, float* important_score,
-                 int32_t* radii, int32_t* num_rendered, void* cuda_stream, bool count_mode, const lgr_raw_params* raw = nullptr)
+                 int32_t* radii, int32_t* num_rendered, void* cuda_stream, bool count_mode, const lgr_raw_params* raw = nullptr,
+                 const lgr_vq_resident_params* vq = nullptr)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    if (vq) {  // resident VQ model: attributes and colour rows come from the compressed arrays (validated by lgr_forward_vq)
+        means3D = vq->xyz;
+        opacities = scales = static_cast<const float*>(vq->attr);
+        rotations = static_cast<const float*>(vq->attr);
+        shs = static_cast<const float*>(vq->codebook);
+    }
     if (raw) {  // fused-activation path: the six leaves replace the activated tensors
         means3D = raw->xyz;
         opacities = raw->opacity;
@@ -1199,17 +1219,24 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
         a.view = v->viewmatrix; a.proj = v->projmatrix; a.campos = v->campos; a.prefiltered = v->prefiltered;
         const int blocks = (P + 255) / 256;
         if (raw) {
-            RawArgs ra;
-            ra.P = P; ra.D = a.D; ra.M = M; ra.W = W; ra.H = H; ra.gx = gx; ra.gy = gy;
-            ra.fx = a.fx; ra.fy = a.fy; ra.tanx = a.tanx; ra.tany = a.tany; ra.mod = a.mod;
-            ra.xyz = raw->xyz; ra.dc = raw->features_dc; ra.rest = raw->features_rest; ra.scaling = raw->scaling;
-            ra.rotation = raw->rotation; ra.opacity = raw->opacity; ra.view = a.view; ra.proj = a.proj; ra.campos = a.campos;
-            ra.prefiltered = a.prefiltered;
+            RawArgs ra = raw_args(a, gx, gy);
+            ra.xyz = raw->xyz;
             ra.rest_stride = raw_rest_stride(raw, M);
+            const LeafSource src = {raw->features_dc, raw->features_rest, raw->scaling, raw->rotation, raw->opacity};
             const size_t smem = raw_smem_bytes_stride(ra.rest_stride);
-            LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_raw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_raw_kernel<LeafSource>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             ProfScope ps(ST_PREPROCESS, stream);
-            preprocess_raw_kernel<<<blocks, 256, smem, stream>>>(ra, radii, geo);
+            preprocess_raw_kernel<<<blocks, 256, smem, stream>>>(ra, src, radii, geo);
+        } else if (vq) {
+            RawArgs ra = raw_args(a, gx, gy);
+            ra.xyz = vq->xyz;
+            ra.rest_stride = (M - 1) * 3;
+            const VqSource src = {vq->attr, vq->slot, static_cast<const __half*>(vq->codebook), vq->nonvq, vq->attr_half, vq->nonvq_half,
+                                  vq->D, vq->Dp, M};
+            const size_t smem = raw_smem_bytes_stride(ra.rest_stride);
+            LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_raw_kernel<VqSource>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ProfScope ps(ST_PREPROCESS, stream);
+            preprocess_raw_kernel<<<blocks, 256, smem, stream>>>(ra, src, radii, geo);
         } else {
             ProfScope ps(ST_PREPROCESS, stream);
             preprocess_kernel<<<blocks, 256, 0, stream>>>(a, radii, geo);
@@ -1410,7 +1437,7 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
     }
     if (count_mode && P > 0) {
         ProfScope ps(ST_SCORE, stream);
-        if (raw) score_from_geom_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, gaussians_count, geo.conic_opacity, important_score);
+        if (raw || vq) score_from_geom_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, gaussians_count, geo.conic_opacity, important_score);
         else score_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, gaussians_count, opacities, important_score);
         LGR_LAUNCH_CHECK("score_kernel", debug, stream);
     }
@@ -1626,6 +1653,49 @@ int lgr_forward_raw(const lgr_view* view, int P, int M, const lgr_raw_params* pa
     return forward_impl(view, P, M, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, geometry_alloc, geometry_user,
                         binning_alloc, binning_user, image_alloc, image_user, out_color, gaussians_count, important_score, radii,
                         num_rendered, cuda_stream, count_mode, params);
+}
+
+int lgr_forward_vq(const lgr_view* view, int P, const lgr_vq_resident_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
+                   lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
+                   int32_t* gaussians_count, float* important_score, int32_t* radii, int32_t* num_rendered, void* cuda_stream)
+{
+    const lgr_vq_resident_params* q = params;
+    if (!q || q->D < 3 || q->D % 3 != 0 || q->D > 48 || q->Dp < q->D || q->Dp % 8 != 0 || q->K < 1) {
+        g_last_error = "lgr_forward_vq: params missing, or D not 3*(degree+1)^2 <= 48, or Dp not a multiple of 8 >= D, or K < 1";
+        return LGR_ERR_INVALID_ARG;
+    }
+    const int M = q->D / 3;
+    if (M != 1 && M != 4 && M != 9 && M != 16) {
+        g_last_error = "lgr_forward_vq: D must be 3*(degree+1)^2";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if ((gaussians_count == nullptr) != (important_score == nullptr)) {
+        g_last_error = "lgr_forward_vq: gaussians_count and important_score must both be NULL or both be set";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P > 0) {
+        const void* dev[] = {q->xyz, q->attr, q->slot, q->codebook, q->nonvq};
+        for (int k = 0; k < 5; k++) {
+            if (!dev[k]) {
+                if (k == 4) continue;  // no non-VQ rows (vq_ratio 1)
+                g_last_error = "lgr_forward_vq: xyz, attr, slot and codebook are required";
+                return LGR_ERR_INVALID_ARG;
+            }
+            cudaPointerAttributes at;
+            if (cudaPointerGetAttributes(&at, dev[k]) != cudaSuccess || at.type != cudaMemoryTypeDevice) {
+                cudaGetLastError();
+                g_last_error = "lgr_forward_vq: every array must be device memory";
+                return LGR_ERR_INVALID_ARG;
+            }
+            if ((uintptr_t)dev[k] & 15) {
+                g_last_error = "lgr_forward_vq: every array must be 16-byte aligned";
+                return LGR_ERR_INVALID_ARG;
+            }
+        }
+    }
+    return forward_impl(view, P, M, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, geometry_alloc, geometry_user,
+                        binning_alloc, binning_user, image_alloc, image_user, out_color, gaussians_count, important_score, radii,
+                        num_rendered, cuda_stream, gaussians_count != nullptr, nullptr, q);
 }
 
 // lgr_backward_raw (one call for both stages, dense outputs) asks stage 1 to clear the gradient rows from inside the blend backward

@@ -337,6 +337,43 @@ def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacit
     return count, score, int(num_rendered.value), out_color, radii, geom, binning, img, leaves
 
 
+def forward_vq_native(count_mode, rs, xyz, store):
+    """Forward of a resident VQ model (lgr_forward_vq): (count, score, color, radii), count and score None unless count_mode.
+    `store` is a vqresident.ResidentVQ; `xyz` its positions ([P,3] float32, the model's _xyz).  No autograd."""
+    lib = capi.load()
+    arrays = (xyz, store.attr, store.slot, store.codebook, store.nonvq)
+    if not all(t.is_cuda and t.device == xyz.device and t.is_contiguous() for t in arrays):
+        raise RuntimeError("forward_vq_native: xyz and the resident arrays must be contiguous tensors on one CUDA device")
+    if xyz.dtype != torch.float32 or tuple(xyz.shape) != (store.P, 3):
+        raise RuntimeError("forward_vq_native: xyz must be float32 [P,3] for the store's P Gaussians")
+    device = xyz.device
+    P, H, W = store.P, int(rs.image_height), int(rs.image_width)
+    out_color = torch.empty((3, H, W), dtype=torch.float32, device=device)
+    radii = torch.empty((P,), dtype=torch.int32, device=device)
+    count = score = None
+    if count_mode:
+        count = torch.empty((P,), dtype=torch.int32, device=device)
+        score = torch.empty((P,), dtype=torch.float32, device=device)
+    params = capi.LgrVqResidentParams(capi.ptr(xyz), capi.ptr(store.attr), capi.ptr(store.slot), capi.ptr(store.codebook),
+                                      capi.ptr(store.nonvq), int(store.attr.dtype == torch.float16),
+                                      int(store.nonvq.dtype == torch.float16), store.D, store.Dp, store.K)
+    slots = [capi.BlobSlot(device) for _ in range(3)]
+    num_rendered = C.c_int32(0)
+    try:
+        with torch.cuda.device(device):
+            view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W, rs.scale_modifier,
+                                    rs.sh_degree, rs.prefiltered, rs.debug)
+            st = lib.lgr_forward_vq(C.byref(view), P, C.byref(params), capi.ALLOC_CB, slots[0].key, capi.ALLOC_CB, slots[1].key,
+                                    capi.ALLOC_CB, slots[2].key, out_color.data_ptr(), capi.ptr(count), capi.ptr(score), capi.ptr(radii),
+                                    C.byref(num_rendered), capi.current_stream_ptr(device))
+        capi.check(st, "lgr_forward_vq")
+    finally:
+        for s_ in slots:
+            s_.release()
+    _last_R[0] = int(num_rendered.value)
+    return count, score, out_color, radii
+
+
 # View-parallel gradient exchange (SURVEY.md section 8e).  When enabled, the backward of the fused node returns gradients that
 # are already SUMMED over all ranks' views: the dense leaves (xyz, scaling, rotation, opacity: 44 B/Gaussian) go through one
 # all-reduce, while the SH gradient (12*M B/Gaussian) is exchanged as its rank-1 factor dRGB (12 B/Gaussian, all-gather) and

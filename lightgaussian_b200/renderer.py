@@ -19,7 +19,7 @@ import torch.nn.functional as F
 from . import trace
 
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rasterize_raw_leaves, fused_activations_match_torch,
-                         rest_row_stride)
+                         rest_row_stride, forward_vq_native)
 
 _LEAVES = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
 
@@ -52,6 +52,27 @@ def _can_fuse(pc, pipe, override_color) -> bool:
     if (pc.active_sh_degree + 1) ** 2 > 1 + pc._features_rest.shape[1]:
         return False
     return fused_activations_match_torch(t.device)
+
+def _resident_store(pc, pipe, override_color):
+    """The resident VQ store of `pc` (vqresident.py) when this call can render the compressed model in place: a forward without
+    gradients, default pipeline flags, SH colours and the standard activations.  Looks only at `pc._vq_resident` and `pc._xyz`, so
+    the deferred leaves stay unread; in every other case the caller's first read of a leaf materialises them."""
+    store = getattr(pc, "_vq_resident", None)
+    if store is None or torch.is_grad_enabled() or override_color is not None:
+        return None
+    if os.environ.get("LGR_FUSED", "1") == "0" or pipe.convert_SHs_python or pipe.compute_cov3D_python:
+        return None
+    if (getattr(pc, "scaling_activation", torch.exp) is not torch.exp or getattr(pc, "opacity_activation", torch.sigmoid) is not torch.sigmoid
+            or getattr(pc, "rotation_activation", F.normalize) is not F.normalize):
+        return None
+    xyz = pc._xyz
+    if not (xyz.is_cuda and xyz.dtype == torch.float32 and xyz.is_contiguous() and tuple(xyz.shape) == (store.P, 3)
+            and xyz.device == store.slot.device):
+        return None
+    if (pc.active_sh_degree + 1) ** 2 > store.D // 3:
+        return None
+    return store if fused_activations_match_torch(xyz.device) else None
+
 
 _SH_C0 = 0.28209479177387814
 _SH_C1 = 0.4886025119029199
@@ -103,6 +124,11 @@ def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_col
         debug=pipe.debug,
         f_count=f_count,
     )
+    store = _resident_store(pc, pipe, override_color)
+    if store is not None:
+        trace.bump("render_vq_resident")
+        count, score, color, radii = forward_vq_native(f_count, settings, pc._xyz.detach(), store)
+        return _package((count, score, color, radii) if f_count else (color, radii), screenspace_points, f_count)
     if _can_fuse(pc, pipe, override_color):
         trace.bump("render_fused")
         if not pc._features_rest.is_contiguous():
