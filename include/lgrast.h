@@ -271,7 +271,9 @@ int lgr_compact_rows(int rows_out, const int32_t* src_row, int n_tensors, const 
  * lgr_vq_assign: idx[i] = argmin_c |x_i - e_c|^2 (evaluated as |e_c|^2 - 2 x_i.e_c like torch.cdist's expansion; smallest index wins
  *   ties).  When cluster_batch / embed_sum are given they receive sum_i w_i [idx_i = c] and sum_i w_i x_i [idx_i = c], with
  *   w_i = weight_i * n / *weight_sum (the reference's normalisation), or 1 when weight is NULL: the quantities EuclideanCodebook.forward
- *   forms with F.one_hot and einsum.  workspace: lgr_vq_workspace_bytes(n) bytes, 8-byte aligned.
+ *   forms with F.one_hot and einsum.  workspace: lgr_vq_workspace_bytes(n) bytes, 8-byte aligned.  The size is the same in every mode:
+ *   it includes the deterministic mode's sort buffers (4 uint32 per sample plus the radix sort's temporary storage, which the function
+ *   queries from CUB on the host), so a workspace stays valid when the mode changes; the default mode uses only the first 8n bytes.
  * lgr_vq_ema_update: cluster_size <- decay*cluster_size + (1-decay)*cluster_batch; embed <- decay*embed + (1-decay)*embed_sum/smoothed,
  *   smoothed = (cluster_size+eps)/(sum+K*eps)*sum (vq.py:286-300).  scratch: one float.
  * lgr_vq_gather: out[i,:] = embed[idx[i],:] (batched_embedding, vq.py:161-165).
@@ -374,6 +376,19 @@ int lgr_set_blend_mode(int mode);
 int lgr_set_binning_mode(int mode);
 uint64_t lgr_binning_overflows(void);
 void lgr_set_binning_estimate(uint64_t instances);   /* overwrite the running estimate of mode 0 (tests; 0 = forget) */
+
+/* Deterministic mode (default off).  On: every output is a function of the inputs alone, whatever the block scheduling, the stream or
+ * other work on the GPU.  The blend backward writes one partial row per (tile, Gaussian) instance, summing the 8 warps of a tile in warp
+ * order, and one pass per Gaussian adds its rows in ascending instance order into the accumulator record (no float atomics, no memset);
+ * lgr_vq_assign's weighted sums come from a stable radix sort of (code, sample) pairs and per-code sums in ascending sample order.
+ * Forward outputs (image, radii, final_T, n_contrib, lists, counts, scores) are bit-identical to the default mode's.  The binning blob
+ * of a forward in this mode is larger: [R][9] floats of partial rows and an R-bit bitmap.  Needs library binning (lgr_set_binning_mode(2))
+ * and the ring blend kernels (lgr_set_blend_mode(0)); any other combination fails with LGR_ERR_INVALID_ARG before any launch.
+ * Process-wide, like the other switches; a backward must run in the mode its forward ran in (the deterministic backward reads the
+ * permutation the deterministic forward stored in its records).  The forward records its mode in geometry header word [10]; a
+ * deterministic backward of a forward that did not run in deterministic mode reads no record and writes NaN into every accumulator,
+ * so all its gradients are NaN (a default backward of a deterministic forward is valid: it ignores the permutation). */
+int lgr_set_deterministic(int on);
 
 /* Diagnostics / A-B: the fused K7+K8 of lgr_backward_raw for a whole view with dense outputs.  0 (default) = one pass zero-fills all
  * output rows (TMA bulk stores) and lists the Gaussians whose accumulators are non-zero, a second kernel runs K7+K8 on that list;

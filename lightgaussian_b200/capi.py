@@ -300,6 +300,17 @@ def set_vq_mode(mode: int) -> None:
     check(load().lgr_set_vq_mode(int(mode)), "lgr_set_vq_mode")
 
 
+def deterministic_requested() -> bool:
+    """The rule every op of this package applies at call time: deterministic mode is on when torch's
+    `torch.use_deterministic_algorithms(True)` is in effect or the environment sets LGR_DETERMINISTIC=1."""
+    return bool(torch.are_deterministic_algorithms_enabled()) or os.environ.get("LGR_DETERMINISTIC", "0") == "1"
+
+
+def set_deterministic(on: bool) -> None:
+    """lgr_set_deterministic: fixed-order reductions in place of the float atomics (process-wide)"""
+    check(load().lgr_set_deterministic(int(bool(on))), "lgr_set_deterministic")
+
+
 def set_kback_mode(mode: int) -> None:
     """fused K7+K8 of the raw backward: 0 = zero-fill + compacted list (default), 1 = dense kernel (A/B measurements)"""
     check(load().lgr_set_kback_mode(int(mode)), "lgr_set_kback_mode")

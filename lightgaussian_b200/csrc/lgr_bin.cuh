@@ -48,7 +48,8 @@ __host__ __device__ inline int bin_pad(int bins) { return (bins + 255) / 256 * 2
 inline int bin_per_block(int P) { return ((P + BIN_V - 1) / BIN_V + 255) / 256 * 256; }
 
 // header words at the start of the geometry blob
-enum { HDR_LISTED = 0, HDR_RENDERED = 1, HDR_CAPACITY = 2, HDR_OVERFLOW = 3, HDR_DONE = 8, HDR_LIVE = 9 };
+// HDR_DET: 1 when the forward ran in deterministic mode (its records carry the permutation the deterministic backward needs)
+enum { HDR_LISTED = 0, HDR_RENDERED = 1, HDR_CAPACITY = 2, HDR_OVERFLOW = 3, HDR_DONE = 8, HDR_LIVE = 9, HDR_DET = 10 };
 
 // lanes with the same key (and valid) get the same mask of lanes; invalid lanes get 0.  One ballot per key bit.
 template <int BITS>

@@ -160,12 +160,15 @@ __device__ __forceinline__ void ring_init(BlendRing& r, int consumers)
 // ------------------------------------------------------------------------------------------------
 // K4/K5 forward
 // ------------------------------------------------------------------------------------------------
-template <bool COUNT, bool STORE>
+// PERM (deterministic mode): word 10 of each stored record is the instance's unsorted index perm[pos], which the deterministic
+// backward uses to address its per-instance partial rows
+template <bool COUNT, bool STORE, bool PERM = false>
 __global__ void __launch_bounds__(BL_THREADS)
 blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H, int tiles_x,
                           const float2* __restrict__ means2D, const float4* __restrict__ conic_opacity, const float4* __restrict__ rgb,
                           const float* __restrict__ bg, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
-                          float* __restrict__ out_color, int* __restrict__ count, float* __restrict__ rec_out, const int* __restrict__ header)
+                          float* __restrict__ out_color, int* __restrict__ count, float* __restrict__ rec_out, const int* __restrict__ header,
+                          const uint32_t* __restrict__ perm = nullptr)
 {
     if (header[HDR_OVERFLOW]) return;   // the binning blob was too small for this view: the host repeats scatter + blend (lgr_bin.cuh)
     __shared__ __align__(128) BlendRing ring;
@@ -202,7 +205,7 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
                 float4* r4 = reinterpret_cast<float4*>(&ring.rec[s][lane * BL_REC]);
                 r4[0] = make_float4(xy.x, xy.y, co.x, co.y);
                 r4[1] = make_float4(co.z, co.w, col.x, col.y);
-                r4[2] = make_float4(col.z, __uint_as_float(id), 0.f, 0.f);
+                r4[2] = make_float4(col.z, __uint_as_float(id), PERM ? __uint_as_float(perm[pos0 + lane]) : 0.f, 0.f);
             }
             if (lane == 0) ring.count[s] = n;
             if (STORE) fence_async_smem();
@@ -309,7 +312,31 @@ struct BlendBackWarp {
     float4 d[32];                  // the lanes' dL/dpix (r, g, b, -)
 };
 
-// contract the buffered pairs of one warp and add them to the accumulator records (see the header comment)
+// Deterministic mode: instead of float atomics, each consumer warp parks its 9 sums of every record it blended in this block of
+// shared memory (per stage, warp and record), and the producer warp adds the 8 warps' sums in warp order once the stage is released.
+struct BlendDetStage {
+    float c[BL_STAGES][8][BL_CH * DET_ROW];
+    uint32_t mask[BL_STAGES][8];   // bit j: the warp wrote record j of the stage's chunk (a culled record counts as zero)
+};
+
+// Where the deterministic regions of a library-path binning blob start (carve_binning with det = true).  Computed from the
+// capacity the blob was sized for, which the backward reads from the geometry header on the device.
+__host__ __device__ __forceinline__ size_t det_partial_offset(size_t Rn)
+{
+    return (Rn * 4 + 255) / 256 * 256 + (Rn * 48 + 255) / 256 * 256;
+}
+__host__ __device__ __forceinline__ size_t det_reached_offset(size_t Rn)
+{
+    return det_partial_offset(Rn) + (Rn * DET_ROW * 4 + 255) / 256 * 256;
+}
+__host__ __device__ __forceinline__ size_t det_ids_offset(size_t Rn)   // ids_unsorted, behind the bitmap
+{
+    return det_reached_offset(Rn) + ((Rn + 31) / 32 * 4 + 255) / 256 * 256;
+}
+
+// contract the buffered pairs of one warp and add them to the accumulator records (see the header comment).  DET: `acc` is the
+// warp's slice of BlendDetStage::c for the current stage and bw.mid holds the record's slot in the chunk; plain stores, no atomics.
+template <bool DET = false>
 __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, int lane, float ox, float oy, float* __restrict__ acc)
 {
     __syncwarp();
@@ -348,7 +375,14 @@ __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, in
     s2xx += __shfl_xor_sync(FULL, s2xx, 16);
     s2xy += __shfl_xor_sync(FULL, s2xy, 16);
     s2yy += __shfl_xor_sync(FULL, s2yy, 16);
-    if (p < nbuf) {
+    if (DET && p < nbuf) {
+        float* row = acc + __float_as_uint(bw.mid[p]) * DET_ROW;
+        if (h == 0) {
+            row[0] = c0; row[1] = c1; row[2] = c2; row[3] = s0; row[4] = s1x;
+        } else {
+            row[5] = s1y; row[6] = s2xx; row[7] = s2xy; row[8] = s2yy;
+        }
+    } else if (p < nbuf) {
         float* rec = acc + (size_t)__float_as_uint(bw.mid[p]) * ACC_STRIDE;
         if (h == 0) {
             atomicAdd(rec + 0, c0);
@@ -366,11 +400,19 @@ __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, in
     __syncwarp();
 }
 
-constexpr size_t blend_back_smem_bytes(bool zero_rows = false)
+constexpr size_t BL_DET_BYTES = (sizeof(BlendDetStage) + 127) / 128 * 128;
+
+constexpr size_t blend_back_smem_bytes(bool zero_rows = false, bool det = false)
 {
-    return (sizeof(BlendRing) + 127) / 128 * 128 + (8 * sizeof(BlendBackWarp) + 127) / 128 * 128 + (zero_rows ? (size_t)KB_ZERO_BYTES : 0);
+    return (sizeof(BlendRing) + 127) / 128 * 128 + (8 * sizeof(BlendBackWarp) + 127) / 128 * 128 + (det ? BL_DET_BYTES : 0) +
+           (zero_rows ? (size_t)KB_ZERO_BYTES : 0);
 }
 
+// DET = false: every (warp, Gaussian) sum goes into acc[id] with float atomics (acc cleared beforehand).
+// DET = true (deterministic mode): the sums of the 8 warps are added in warp order per record and written as one partial row per
+// instance, at the instance's unsorted index (record word 10), into the binning blob; det_gather_kernel then adds each Gaussian's rows
+// in ascending unsorted-index order.  The bitmap behind the rows marks the instances that got a row.  No float atomics.
+template <bool DET = false>
 __global__ void __launch_bounds__(BL_THREADS)
 blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_blob, const int* __restrict__ header, int W, int H,
                            int tiles_x, const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
@@ -379,12 +421,14 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
     extern __shared__ __align__(128) unsigned char blend_dyn_smem[];
     BlendRing& ring = *reinterpret_cast<BlendRing*>(blend_dyn_smem);
     BlendBackWarp* warps = reinterpret_cast<BlendBackWarp*>(blend_dyn_smem + ((sizeof(BlendRing) + 127) / 128) * 128);
+    unsigned char* behind_warps = reinterpret_cast<unsigned char*>(warps) + (8 * sizeof(BlendBackWarp) + 127) / 128 * 128;
+    BlendDetStage* det = reinterpret_cast<BlendDetStage*>(behind_warps);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x;
     const uint2 range = ranges[tile];
     // zero.P > 0: this launch also clears the dense gradient rows K7+K8 will (sparsely) write -- a page of zeros behind the per-warp
     // buffers, one thread, a handful of bulk stores per tile; the HBM writes overlap the blend, which leaves DRAM ~97 % idle
-    float* zero_page = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(warps) + (8 * sizeof(BlendBackWarp) + 127) / 128 * 128);
+    float* zero_page = reinterpret_cast<float*>(behind_warps + (DET ? BL_DET_BYTES : 0));
     const bool zero_rows = zero.P > 0;
     if (zero_rows) {
         for (int k = threadIdx.x; k < KB_ZERO_BYTES / 4; k += BL_THREADS) zero_page[k] = 0.f;
@@ -404,12 +448,63 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
     if (lane == 0 && warp_max) atomicMax(&ring.tile_max, warp_max);
     __syncthreads();
     const uint32_t tile_max = ring.tile_max;
-    if (tile_max == 0) {
+    // DET: a forward that did not run in deterministic mode stored no permutation; nothing is read or written (det_gather_kernel then
+    // writes NaN accumulators, so the misuse shows in every gradient instead of corrupting memory)
+    if (tile_max == 0 || (DET && header[HDR_DET] != 1)) {
         if (zero_rows && threadIdx.x == 8 * 32) bulk_wait_all();   // the zero page must outlive the stores that read it
         return;
     }
     const uint32_t nchunks = (tile_max + BL_CH - 1) / BL_CH;
 
+    if (DET && warp == 8) {
+        // ===== producer, deterministic mode: lane 0 streams the records as below; before a stage is refilled (and for the last
+        // BL_STAGES chunks after the loads), the whole warp adds the consumers' sums of the chunk it held, lane j for record j =====
+        const size_t Rn = (size_t)max(header[HDR_CAPACITY], 1);
+        const float* rec_in = reinterpret_cast<const float*>(binning_blob + (Rn * 4 + 255) / 256 * 256);
+        float* partial = reinterpret_cast<float*>(const_cast<char*>(binning_blob) + det_partial_offset(Rn));
+        uint32_t* reached = reinterpret_cast<uint32_t*>(const_cast<char*>(binning_blob) + det_reached_offset(Rn));
+        for (uint32_t i = 0; i < nchunks + BL_STAGES; i++) {
+            const int s = i % BL_STAGES;
+            const uint32_t ph = (i / BL_STAGES) & 1u;
+            if (i >= BL_STAGES) {
+                mbar_wait_ring(&ring.empty[s], ph ^ 1u);   // all 8 warps released chunk i - BL_STAGES
+                const uint32_t b = nchunks - 1 - (i - BL_STAGES);
+                const uint32_t n = min((uint32_t)BL_CH, tile_max - b * BL_CH);
+                if ((uint32_t)lane < n) {
+                    const uint32_t u = __float_as_uint(ring.rec[s][lane * BL_REC + 10]);
+                    float v[DET_ROW];
+#pragma unroll
+                    for (int k = 0; k < DET_ROW; k++) v[k] = 0.f;
+#pragma unroll
+                    for (int w = 0; w < 8; w++) {
+                        if ((det->mask[s][w] >> lane) & 1u) {
+                            const float* c = &det->c[s][w][lane * DET_ROW];
+#pragma unroll
+                            for (int k = 0; k < DET_ROW; k++) v[k] += c[k];
+                        }
+                    }
+                    if (u < Rn) {
+#pragma unroll
+                        for (int k = 0; k < DET_ROW; k++) partial[(size_t)u * DET_ROW + k] = v[k];
+                        atomicOr(&reached[u >> 5], 1u << (u & 31));
+                    }
+                }
+                __syncwarp();
+            }
+            if (i >= nchunks) continue;
+            if (lane == 0) {
+                if (i < BL_STAGES) mbar_wait_ring(&ring.empty[s], ph ^ 1u);
+                const uint32_t b = nchunks - 1 - i;
+                const uint32_t n = min((uint32_t)BL_CH, tile_max - b * BL_CH);
+                const uint32_t bytes = n * (uint32_t)(BL_REC * 4);
+                mbar_expect_tx(&ring.full[s], bytes);
+                bulk_g2s(&ring.rec[s][0], rec_in + ((size_t)range.x + (size_t)b * BL_CH) * BL_REC, bytes, &ring.full[s]);
+            }
+            __syncwarp();
+        }
+        if (zero_rows && lane == 0) bulk_wait_all();
+        return;
+    }
     if (warp == 8) {
         // ===== producer: one thread streams the records back to front with TMA bulk loads =====
         if (lane == 0) {
@@ -457,6 +552,8 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
         const int s = i % BL_STAGES;
         const uint32_t ph = (i / BL_STAGES) & 1u;
         mbar_wait_ring(&ring.full[s], ph);
+        uint32_t wrote = 0;   // DET: records of this chunk with a parked row
+        float* parked = DET ? &det->c[s][warp][0] : acc;
         if (b * BL_CH < warp_max) {
             const float* stage = &ring.rec[s][0];
             const uint32_t n = min((uint32_t)BL_CH, tile_max - b * BL_CH);
@@ -496,20 +593,67 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
                 bw.w[nbuf][lane] = w;
                 bw.g[nbuf][lane] = G * dL_dalpha;
                 if (lane == 0) {
-                    bw.mid[nbuf] = q2.y;
+                    bw.mid[nbuf] = DET ? __uint_as_float((uint32_t)j) : q2.y;
                     bw.mgx[nbuf] = q0.x;
                     bw.mgy[nbuf] = q0.y;
                 }
+                if (DET) wrote |= 1u << j;
                 if (++nbuf == BL_FLUSH) {
-                    back_flush(bw, nbuf, lane, rx0, ry0, acc);
+                    back_flush<DET>(bw, nbuf, lane, rx0, ry0, parked);
                     nbuf = 0;
                 }
             }
         }
+        if (DET) {   // every row of this chunk is parked before the stage is released
+            if (nbuf) back_flush<DET>(bw, nbuf, lane, rx0, ry0, parked);
+            nbuf = 0;
+            if (lane == 0) det->mask[s][warp] = wrote;
+            __threadfence_block();
+        }
         __syncwarp();
         if (lane == 0) mbar_arrive(&ring.empty[s]);
     }
-    if (nbuf) back_flush(bw, nbuf, lane, rx0, ry0, acc);
+    if (!DET && nbuf) back_flush(bw, nbuf, lane, rx0, ry0, acc);
+}
+
+// ---- deterministic mode, across tiles: the Gaussian of depth rank k owns the unsorted instances [offsets[k-1], offsets[k]) (emit
+// order: row-major tiles of its rectangle).  Thread t adds the partial rows of rank t's instances in ascending unsorted-index order and
+// writes that Gaussian's whole accumulator record, and writes a zero record for Gaussian t if it has no instance.  Replaces the memset +
+// atomics.  Reads only what the forward left (tiles_kept, offsets, the blob's ids_unsorted), not sorted_ids, which K7+K8 reuses.
+__global__ void __launch_bounds__(256)
+det_gather_kernel(int P, const uint32_t* __restrict__ tiles_kept, const unsigned long long* __restrict__ offsets,
+                  const char* __restrict__ binning_blob, const int* __restrict__ header, float* __restrict__ acc)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= P) return;
+    if (header[HDR_DET] != 1) {   // the forward did not run in deterministic mode: refuse with NaN rather than read foreign data
+        float4* rec = reinterpret_cast<float4*>(acc + (size_t)t * ACC_STRIDE);
+        rec[0] = rec[1] = rec[2] = make_float4(__int_as_float(0x7fc00000), __int_as_float(0x7fc00000), __int_as_float(0x7fc00000), 0.f);
+        return;
+    }
+    if (tiles_kept[t] == 0) {
+        float4* rec = reinterpret_cast<float4*>(acc + (size_t)t * ACC_STRIDE);
+        rec[0] = rec[1] = rec[2] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    const uint32_t end = (uint32_t)offsets[t], begin = t ? (uint32_t)offsets[t - 1] : 0u;
+    if (end == begin) return;
+    const size_t Rn = (size_t)max(header[HDR_CAPACITY], 1);
+    const float* partial = reinterpret_cast<const float*>(binning_blob + det_partial_offset(Rn));
+    const uint32_t* reached = reinterpret_cast<const uint32_t*>(binning_blob + det_reached_offset(Rn));
+    const uint32_t* ids_unsorted = reinterpret_cast<const uint32_t*>(binning_blob + det_ids_offset(Rn));
+    float v[DET_ROW];
+#pragma unroll
+    for (int q = 0; q < DET_ROW; q++) v[q] = 0.f;
+    for (uint32_t u = begin; u < end; u++) {
+        if (!((reached[u >> 5] >> (u & 31)) & 1u)) continue;   // never walked by the backward: contributes exactly zero
+        const float* r = partial + (size_t)u * DET_ROW;
+#pragma unroll
+        for (int q = 0; q < DET_ROW; q++) v[q] += r[q];
+    }
+    float4* rec = reinterpret_cast<float4*>(acc + (size_t)ids_unsorted[begin] * ACC_STRIDE);
+    rec[0] = make_float4(v[0], v[1], v[2], v[3]);
+    rec[1] = make_float4(v[4], v[5], v[6], v[7]);
+    rec[2] = make_float4(v[8], 0.f, 0.f, 0.f);
 }
 
 }  // namespace

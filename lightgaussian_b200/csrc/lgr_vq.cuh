@@ -139,6 +139,71 @@ vq_accumulate_kernel(int n, int d, const unsigned long long* __restrict__ best, 
     }
 }
 
+// ---- deterministic mode: the same sums without float atomics.  A stable radix sort of (code, sample) pairs groups the samples of each
+// code in ascending sample order; one warp per code then adds them in that order. ----
+__global__ void __launch_bounds__(256)
+vq_det_keys_kernel(int n, const unsigned long long* __restrict__ best, int* __restrict__ idx_out, uint32_t* __restrict__ codes,
+                   uint32_t* __restrict__ rows)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t c = (uint32_t)best[i];
+    if (idx_out) idx_out[i] = (int)c;
+    codes[i] = c;
+    rows[i] = (uint32_t)i;
+}
+
+// block = code c: segment [lower(c), lower(c+1)) of the sorted codes.  Warp w adds the samples a+w, a+w+VQ_SEG_WARPS, ... in that order
+// (lane l owns columns l, l+32, l+64 of [embed_sum row | batch], column d being cluster_batch); the warps' partial sums are then added
+// in warp order.  The split depends only on the sorted order, so the result is deterministic, and a code that holds every sample is
+// added by VQ_SEG_WARPS warps instead of one.  Every code's sums are written, zero for a code no sample chose.
+constexpr int VQ_SEG_WARPS = 8;
+__global__ void __launch_bounds__(VQ_SEG_WARPS * 32)
+vq_det_segsum_kernel(int n, int d, int K, const uint32_t* __restrict__ codes, const uint32_t* __restrict__ rows, const float* __restrict__ x,
+                     const float* __restrict__ weight, float weight_numel, const float* __restrict__ weight_sum, float* __restrict__ cluster_batch,
+                     float* __restrict__ embed_sum)
+{
+    __shared__ float part[VQ_SEG_WARPS][96];
+    __shared__ int seg[2];
+    const int c = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x < 2) {
+        const uint32_t key = (uint32_t)c + (uint32_t)threadIdx.x;
+        int lo = 0, hi = n;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (codes[mid] < key) lo = mid + 1;
+            else hi = mid;
+        }
+        seg[threadIdx.x] = lo;
+    }
+    __syncthreads();
+    const int a = seg[0], b = seg[1];
+    float acc[3] = {0.f, 0.f, 0.f};
+    for (int k = a + warp; k < b; k += VQ_SEG_WARPS) {
+        const int i = (int)rows[k];
+        const float w = weight ? __fdiv_rn(__fmul_rn(weight[i], weight_numel), weight_sum[0]) : 1.0f;   // as vq_accumulate_kernel
+#pragma unroll
+        for (int q = 0; q < 3; q++) {
+            const int j = lane + 32 * q;
+            if (j < d) acc[q] = __fadd_rn(acc[q], __fmul_rn(x[(size_t)i * d + j], w));
+            else if (j == d) acc[q] = __fadd_rn(acc[q], w);
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < 3; q++) part[warp][lane + 32 * q] = acc[q];
+    __syncthreads();
+    for (int j = threadIdx.x; j <= d; j += blockDim.x) {
+        float v = 0.f;
+#pragma unroll
+        for (int w = 0; w < VQ_SEG_WARPS; w++) v = __fadd_rn(v, part[w][j]);
+        if (j < d) {
+            if (embed_sum) embed_sum[(size_t)c * d + j] = v;
+        } else if (cluster_batch) {
+            cluster_batch[c] = v;
+        }
+    }
+}
+
 // one block: cluster_size EMA and its total (fixed summation order -> deterministic given the batch sums)
 __global__ void __launch_bounds__(1024)
 vq_ema_cluster_kernel(int K, float decay, float one_minus_decay, float* __restrict__ cluster_size, const float* __restrict__ cluster_batch,

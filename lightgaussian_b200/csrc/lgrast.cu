@@ -41,6 +41,7 @@ namespace {
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int LGR_SMS = 132;    // streaming multiprocessors of an H100 SXM: grid sizes of the grid-stride kernels
 constexpr int ACC_STRIDE = 12;  // floats per Gaussian in the backward accumulator record
+constexpr int DET_ROW = 9;      // floats per partial row of the deterministic blend backward: the record without its pad
 // record layout: 0..2 dL/dcolor rgb | 3 S0 | 4,5 S1x,S1y | 6,7,8 S2xx,S2xy,S2yy | 9..11 pad
 // with w = G * dL/dalpha per (pixel, Gaussian) pair and d = mean2D - pixel:  S0 = sum w, S1 = sum w*d, S2 = sum w*d*d^T.
 // The per-Gaussian factors (conic, opacity, viewport) are applied once per Gaussian in K8 (accum_to_grad2d).
@@ -54,19 +55,22 @@ int g_blend_mode = 0;   // 0 = ring kernels (lgr_blend.cuh), 1 = round-1 kernels
 int g_bin_mode = 2;
 std::atomic<size_t> g_bin_hint{0};   // running estimate of the listed instances per view (mode 0)
 int g_vq_mode = 0;      // VecTree nearest-code search: 0 = tensor-core coarse pass + exact FP32 rescore (d <= 32), 1 = FP32 FFMA kernel only
+// deterministic mode (lgr_set_deterministic): fixed-order reductions in place of the float atomics of the blend backward and the VecTree
+// accumulation; needs library binning and the ring blend kernels
+int g_det = 0;
 int g_kback_mode = 0;   // single-GPU K7+K8: 0 = rows cleared inside the blend backward + compacted list (lgr_sparse.cuh), 1 = dense kernel, 2 = separate zero-fill kernel + compacted list (A/B)
 std::atomic<uint64_t> g_launches{0};
 
 // ---- optional per-stage device timing (CUDA events on the launch stream), used by bench.py's roofline ----
 enum StageId { ST_PREPROCESS = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_TILE_SORT, ST_RANGES, ST_BLEND_FWD, ST_BLEND_FWD_COUNT,
-               ST_SCORE, ST_BLEND_BWD, ST_PREPROCESS_BWD, ST_MEMSET, ST_SH_GRAD, ST_PEER_ALLREDUCE, ST_LOSS_FWD, ST_LOSS_BWD, ST_ADAMW, ST_COMPACT, ST_VQ_ASSIGN, ST_VQ_UPDATE, ST_SPARSE_PACK, ST_SPARSE_ACC, ST_BIN_DSORT, ST_BIN_COUNT, ST_BIN_SCATTER, ST_COUNT };
+               ST_SCORE, ST_BLEND_BWD, ST_PREPROCESS_BWD, ST_MEMSET, ST_SH_GRAD, ST_PEER_ALLREDUCE, ST_LOSS_FWD, ST_LOSS_BWD, ST_ADAMW, ST_COMPACT, ST_VQ_ASSIGN, ST_VQ_UPDATE, ST_SPARSE_PACK, ST_SPARSE_ACC, ST_BIN_DSORT, ST_BIN_COUNT, ST_BIN_SCATTER, ST_DET_GATHER, ST_COUNT };
 const char* const kStageNames[ST_COUNT] = {"preprocess_kernel", "depth_sort(cub)", "scan(cub)", "emit_kernel", "tile_sort(cub)",
                                            "ranges_kernel", "blend_forward_kernel", "blend_forward_kernel<count>", "score_kernel",
                                            "blend_backward_kernel", "preprocess_backward_kernel", "memset", "sh_grad_from_views_kernel",
                                            "peer_allreduce_kernel", "image_loss_forward_kernel", "image_loss_backward_kernel", "adamw_multi_kernel",
                                            "compact_gather_kernel", "vq_assign_kernel", "vq_ema_kernels", "sparse_pack(flag+scan+index+K8)",
                                            "sparse_accumulate_kernel", "depth_sort(dsort_count+bin_scan+dsort_scatter x3)", "tile_count_kernel+bin_scan_kernel",
-                                           "tile_scatter_kernel"};
+                                           "tile_scatter_kernel", "det_gather_kernel"};
 struct ProfRecord { int stage; cudaEvent_t a, b; };
 bool g_prof_on = false;
 std::vector<ProfRecord> g_prof_records;
@@ -271,13 +275,18 @@ struct BinningState {
     char* cub_temp;
     size_t cub_temp_bytes;
     float* records;             // [R][12] per-instance records in list order, written by the forward blend for the chunks it visits
+    float* det_partial;         // deterministic mode: [R][9] partial rows by unsorted index (forward: [R] sorted -> unsorted permutation)
+    uint32_t* det_reached;      // deterministic mode: [ceil(R/32)] bit u = the backward wrote partial row u
     bool wide_keys;
     size_t offs[1];
     size_t total;
 };
 
 // R = instances the blob holds: the listed count on the library path and in mode 1, the capacity estimate in mode 0
-BinningState carve_binning(char* base, size_t R, int W, int H, bool library_binning)
+// det (deterministic mode, library binning only): the per-instance partial rows of the backward ([R][9] floats, which hold the sort's
+// permutation during the forward) and a bitmap of the instances the backward reached follow the records; det_*_offset (lgr_blend.cuh)
+// recompute these offsets on the device
+BinningState carve_binning(char* base, size_t R, int W, int H, bool library_binning, bool det = false)
 {
     BinningState b;
     const int bits = tile_key_bits(W, H);
@@ -287,9 +296,14 @@ BinningState carve_binning(char* base, size_t R, int W, int H, bool library_binn
     b.point_list = c.take<uint32_t>(Rn, &b.offs[0]);
     b.records = c.take<float>(Rn * 12);   // second region: its offset, align_up(4*max(R,1), 256), is recomputed ON THE DEVICE by the backward
     b.ids_unsorted = nullptr; b.keys_unsorted = b.keys_sorted = nullptr; b.cub_temp = nullptr; b.cub_temp_bytes = 0;
+    b.det_partial = nullptr; b.det_reached = nullptr;
     if (!library_binning) {
         b.total = align_up(c.off, 256);
         return b;
+    }
+    if (det) {
+        b.det_partial = c.take<float>(Rn * DET_ROW);
+        b.det_reached = c.take<uint32_t>((Rn + 31) / 32);
     }
     b.ids_unsorted = c.take<uint32_t>(Rn);
     const size_t ksz = b.wide_keys ? 4 : 2;
@@ -1107,11 +1121,12 @@ struct SyncEvent {
 thread_local SyncEvent t_event;
 std::atomic<uint64_t> g_bin_overflows{0};
 
-__global__ void set_capacity_kernel(int* header, int capacity)
+__global__ void set_capacity_kernel(int* header, int capacity, int det)
 {
     if (threadIdx.x == 0) {
         header[HDR_CAPACITY] = capacity;
         header[HDR_OVERFLOW] = 0;
+        header[HDR_DET] = det;
     }
 }
 
@@ -1125,6 +1140,53 @@ inline RawArgs raw_args(const PreprocessArgs& a, int gx, int gy)
     ra.prefiltered = a.prefiltered;
     ra.rest_stride = 0;
     return ra;
+}
+
+// deterministic mode: the binning's helpers (iota as sort values, point_list by gather through the permutation)
+__global__ void __launch_bounds__(256) det_iota_kernel(int R, uint32_t* __restrict__ out)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < R) out[i] = (uint32_t)i;
+}
+__global__ void __launch_bounds__(256) det_point_list_kernel(int R, const uint32_t* __restrict__ perm, const uint32_t* __restrict__ ids_unsorted,
+                                                             uint32_t* __restrict__ point_list)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < R) point_list[i] = ids_unsorted[perm[i]];
+}
+
+// Deterministic mode's tile sort: the values are the unsorted instance indices, so the stable sort yields the permutation (sorted ->
+// unsorted), which the forward blend stores in the records for the deterministic backward; the ids follow by one gather, the same list
+// as sorting the ids themselves.  The permutation lives in the partial-row region until the backward overwrites it.  Also clears the
+// bitmap of instances the backward reaches.
+template <typename KeyT>
+int det_tile_sort(const BinningState& bin, int R, int bits, bool debug, cudaStream_t stream)
+{
+    uint32_t* perm = reinterpret_cast<uint32_t*>(bin.det_partial);
+    det_iota_kernel<<<(R + 255) / 256, 256, 0, stream>>>(R, bin.point_list);
+    LGR_LAUNCH_CHECK("det_iota_kernel", debug, stream);
+    size_t tmp = bin.cub_temp_bytes;
+    LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const KeyT*)bin.keys_unsorted, (KeyT*)bin.keys_sorted,
+                                                  (const uint32_t*)bin.point_list, perm, R, 0, bits, stream));
+    det_point_list_kernel<<<(R + 255) / 256, 256, 0, stream>>>(R, perm, bin.ids_unsorted, bin.point_list);
+    LGR_LAUNCH_CHECK("det_point_list_kernel", debug, stream);
+    LGR_CUDA_TRY(cudaMemsetAsync(bin.det_reached, 0, sizeof(uint32_t) * (((size_t)R + 31) / 32), stream));
+    return LGR_OK;
+}
+
+// deterministic mode has no implementation for the hand-written binning or the round-1 blend kernels: refuse before any launch
+bool det_supported(const char* what)
+{
+    if (g_bin_mode != 2) {
+        g_last_error = std::string(what) + ": deterministic mode needs library binning; lgr_set_binning_mode(" + std::to_string(g_bin_mode) +
+                       ") has no deterministic implementation";
+        return false;
+    }
+    if (g_blend_mode != 0) {
+        g_last_error = std::string(what) + ": deterministic mode needs the ring blend kernels; lgr_set_blend_mode(1) has no deterministic implementation";
+        return false;
+    }
+    return true;
 }
 
 int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const float* shs, const float* colors_precomp,
@@ -1183,6 +1245,7 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
             return LGR_ERR_INVALID_ARG;
         }
     }
+    if (g_det && !det_supported("lgr_forward")) return LGR_ERR_INVALID_ARG;
     const bool debug = v->debug != 0;
     *num_rendered = 0;
     const int gx = (W + LGR_TILE - 1) / LGR_TILE, gy = (H + LGR_TILE - 1) / LGR_TILE;
@@ -1246,6 +1309,7 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
 
     int R = 0, R_ref = 0;
     BinningState bin = {};
+    const bool det = g_det != 0;   // lib_bin holds: det_supported() refused the hand-written binning
     int* host_hdr = t_pinned.get();
 
     // K4/K5 -- and everything of it that has to be repeated when the binning blob turns out too small
@@ -1256,6 +1320,11 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
             blend_forward_ring_kernel<true, false><<<tiles, BL_THREADS, 0, stream>>>(img.ranges, bin.point_list, W, H, gx, geo.means2D, geo.conic_opacity,
                                                                                       geo.rgb, v->background, img.final_T, img.n_contrib, out_color,
                                                                                       gaussians_count, nullptr, geo.num_rendered);
+        else if (g_blend_mode == 0 && det)
+            blend_forward_ring_kernel<false, true, true><<<tiles, BL_THREADS, 0, stream>>>(img.ranges, bin.point_list, W, H, gx, geo.means2D,
+                                                                                            geo.conic_opacity, geo.rgb, v->background, img.final_T,
+                                                                                            img.n_contrib, out_color, nullptr, bin.records,
+                                                                                            geo.num_rendered, reinterpret_cast<const uint32_t*>(bin.det_partial));
         else if (g_blend_mode == 0)
             blend_forward_ring_kernel<false, true><<<tiles, BL_THREADS, 0, stream>>>(img.ranges, bin.point_list, W, H, gx, geo.means2D, geo.conic_opacity,
                                                                                       geo.rgb, v->background, img.final_T, img.n_contrib, out_color,
@@ -1334,7 +1403,7 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
             char* bin_blob = binning_alloc(binning_user, bin.total);
             if (!bin_blob) { g_last_error = "binning allocator returned NULL"; return LGR_ERR_ALLOC; }
             bin = carve_binning(bin_blob, (size_t)R, W, H, false);
-            set_capacity_kernel<<<1, 32, 0, stream>>>(geo.num_rendered, R > 0 ? R : 1);
+            set_capacity_kernel<<<1, 32, 0, stream>>>(geo.num_rendered, R > 0 ? R : 1, 0);
             LGR_LAUNCH_CHECK("set_capacity_kernel", debug, stream);
             return LGR_OK;
         };
@@ -1388,11 +1457,11 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
         LGR_CUDA_TRY(cudaStreamSynchronize(stream));
         R = host_hdr[0];       // instances actually emitted (after exact tile culling)
         R_ref = host_hdr[1];   // the reference's num_rendered: sum of the tile-rectangle areas
-        bin = carve_binning(nullptr, (size_t)R, W, H, true);
+        bin = carve_binning(nullptr, (size_t)R, W, H, true, det);
         char* bin_blob = binning_alloc(binning_user, bin.total);
         if (!bin_blob) { g_last_error = "binning allocator returned NULL"; return LGR_ERR_ALLOC; }
-        bin = carve_binning(bin_blob, (size_t)R, W, H, true);
-        set_capacity_kernel<<<1, 32, 0, stream>>>(geo.num_rendered, R > 0 ? R : 1);
+        bin = carve_binning(bin_blob, (size_t)R, W, H, true, det);
+        set_capacity_kernel<<<1, 32, 0, stream>>>(geo.num_rendered, R > 0 ? R : 1, det ? 1 : 0);
         LGR_LAUNCH_CHECK("set_capacity_kernel", debug, stream);
 
         if (R > 0) {
@@ -1408,9 +1477,13 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
                 LGR_LAUNCH_CHECK("emit_kernel", debug, stream);
                 {
                     ProfScope ps(ST_TILE_SORT, stream);
-                    LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const uint32_t*)bin.keys_unsorted,
-                                                                  (uint32_t*)bin.keys_sorted, (const uint32_t*)bin.ids_unsorted,
-                                                                  bin.point_list, R, 0, bits, stream));
+                    if (det) {
+                        const int st = det_tile_sort<uint32_t>(bin, R, bits, debug, stream);
+                        if (st != LGR_OK) return st;
+                    } else
+                        LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const uint32_t*)bin.keys_unsorted,
+                                                                      (uint32_t*)bin.keys_sorted, (const uint32_t*)bin.ids_unsorted,
+                                                                      bin.point_list, R, 0, bits, stream));
                 }
                 ProfScope ps(ST_RANGES, stream);
                 ranges_kernel<uint32_t><<<(gx * gy + 255) / 256, 256, 0, stream>>>(R, gx * gy, (const uint32_t*)bin.keys_sorted, img.ranges);
@@ -1423,9 +1496,13 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
                 LGR_LAUNCH_CHECK("emit_kernel", debug, stream);
                 {
                     ProfScope ps(ST_TILE_SORT, stream);
-                    LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const uint16_t*)bin.keys_unsorted,
-                                                                  (uint16_t*)bin.keys_sorted, (const uint32_t*)bin.ids_unsorted,
-                                                                  bin.point_list, R, 0, bits, stream));
+                    if (det) {
+                        const int st = det_tile_sort<uint16_t>(bin, R, bits, debug, stream);
+                        if (st != LGR_OK) return st;
+                    } else
+                        LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const uint16_t*)bin.keys_unsorted,
+                                                                      (uint16_t*)bin.keys_sorted, (const uint32_t*)bin.ids_unsorted,
+                                                                      bin.point_list, R, 0, bits, stream));
                 }
                 ProfScope ps(ST_RANGES, stream);
                 ranges_kernel<uint16_t><<<(gx * gy + 255) / 256, 256, 0, stream>>>(R, gx * gy, (const uint16_t*)bin.keys_sorted, img.ranges);
@@ -1443,6 +1520,30 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
     }
     (void)N;
     *num_rendered = R_ref;
+    return LGR_OK;
+}
+
+// Deterministic stage 1 of every backward: blend backward with fixed-order sums into per-instance partial rows, then one pass per
+// Gaussian that writes every accumulator record (no memset, no float atomics).  zr.P > 0: the blend backward also clears the dense
+// gradient rows, exactly as the default kernel does for kback mode 0.
+int blend_backward_det(const GeometryState& geo, const ImageState& img, char* binning_blob, int P, int W, int H, const float* background,
+                       const float* dL_dout_color, const KbackZeroArgs& zr, bool debug, cudaStream_t stream)
+{
+    const int gx = (W + LGR_TILE - 1) / LGR_TILE, gy = (H + LGR_TILE - 1) / LGR_TILE;
+    {
+        ProfScope ps(ST_BLEND_BWD, stream);
+        const size_t bsmem = blend_back_smem_bytes(zr.P > 0, true);
+        LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)blend_back_smem_bytes(true, true)));
+        blend_backward_ring_kernel<true><<<gx * gy, BL_THREADS, bsmem, stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx, background,
+                                                                                  img.final_T, img.n_contrib, dL_dout_color, geo.grad_acc, zr);
+        LGR_LAUNCH_CHECK("blend_backward_ring_kernel<det>", debug, stream);
+    }
+    {
+        ProfScope ps(ST_DET_GATHER, stream);
+        det_gather_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, geo.tiles_kept, geo.offsets, binning_blob, geo.num_rendered, geo.grad_acc);
+        LGR_LAUNCH_CHECK("det_gather_kernel", debug, stream);
+    }
     return LGR_OK;
 }
 
@@ -1471,6 +1572,12 @@ int lgr_set_binning_mode(int mode)
         return LGR_ERR_INVALID_ARG;
     }
     g_bin_mode = mode;
+    return LGR_OK;
+}
+
+int lgr_set_deterministic(int on)
+{
+    g_det = on != 0;
     return LGR_OK;
 }
 
@@ -1597,24 +1704,28 @@ int lgr_backward(const lgr_view* v, int P, int M, int num_rendered, const float*
         g_last_error = "lgr_backward: rotations, shs, dL_dsh and dL_drotations must be 16-byte aligned";
         return LGR_ERR_INVALID_ARG;
     }
+    if (g_det && !det_supported("lgr_backward")) return LGR_ERR_INVALID_ARG;
     const bool debug = v->debug != 0;
     const int W = v->image_width, H = v->image_height;
     const int gx = (W + LGR_TILE - 1) / LGR_TILE, gy = (H + LGR_TILE - 1) / LGR_TILE;
-    GeometryState geo = carve_geometry(geometry_blob, (size_t)P, false);
+    GeometryState geo = carve_geometry(geometry_blob, (size_t)P, g_det != 0);
     ImageState img = carve_image(image_blob, W, H, false);
     BinningState bin = carve_binning(binning_blob, (size_t)(num_rendered > 0 ? num_rendered : 0), W, H, false);
 
-    {
+    if (g_det) {
+        const int st = blend_backward_det(geo, img, binning_blob, P, W, H, v->background, dL_dout_color, KbackZeroArgs{}, debug, stream);
+        if (st != LGR_OK) return st;
+    } else {
         ProfScope ps(ST_MEMSET, stream);
         LGR_CUDA_TRY(cudaMemsetAsync(geo.grad_acc, 0, sizeof(float) * ACC_STRIDE * (size_t)P, stream));
     }
-    if (num_rendered > 0) {
+    if (num_rendered > 0 && !g_det) {
         ProfScope ps(ST_BLEND_BWD, stream);
         if (g_blend_mode == 0) {
-            LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes()));
+            LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes()));
             // the host only knows the reference's num_rendered here; the number of LISTED instances (which fixes where the records
             // start inside the binning blob) sits in the geometry header on the device
-            blend_backward_ring_kernel<<<gx * gy, BL_THREADS, blend_back_smem_bytes(), stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
+            blend_backward_ring_kernel<false><<<gx * gy, BL_THREADS, blend_back_smem_bytes(), stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
                                                                                                    v->background, img.final_T, img.n_contrib,
                                                                                                    dL_dout_color, geo.grad_acc, KbackZeroArgs{});
         } else
@@ -1712,27 +1823,34 @@ int lgr_backward_raw_begin(const lgr_view* v, int P, int num_rendered, const int
         g_last_error = "lgr_backward_raw_begin: missing required argument";
         return LGR_ERR_INVALID_ARG;
     }
+    if (g_det && !det_supported("lgr_backward_raw")) { t_zero_req.P = 0; return LGR_ERR_INVALID_ARG; }
     const bool debug = v->debug != 0;
     const int W = v->image_width, H = v->image_height;
     const int gx = (W + LGR_TILE - 1) / LGR_TILE, gy = (H + LGR_TILE - 1) / LGR_TILE;
-    GeometryState geo = carve_geometry(geometry_blob, (size_t)P, false);
+    GeometryState geo = carve_geometry(geometry_blob, (size_t)P, g_det != 0);
     ImageState img = carve_image(image_blob, W, H, false);
     BinningState bin = carve_binning(binning_blob, (size_t)(num_rendered > 0 ? num_rendered : 0), W, H, false);
-    {
+    if (g_det) {
+        const KbackZeroArgs zr = t_zero_req;
+        t_zero_req.P = 0;
+        const int st = blend_backward_det(geo, img, binning_blob, P, W, H, v->background, dL_dout_color, zr, debug, stream);
+        if (st != LGR_OK) return st;
+        t_rows_zeroed = zr.P > 0;
+    } else {
         ProfScope ps(ST_MEMSET, stream);
         LGR_CUDA_TRY(cudaMemsetAsync(geo.grad_acc, 0, sizeof(float) * ACC_STRIDE * (size_t)P, stream));
     }
-    if (num_rendered > 0) {
+    if (num_rendered > 0 && !g_det) {
         ProfScope ps(ST_BLEND_BWD, stream);
         if (g_blend_mode == 0) {
-            LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes()));
+            LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes()));
             // the host only knows the reference's num_rendered here; the number of LISTED instances (which fixes where the records
             // start inside the binning blob) sits in the geometry header on the device
             const KbackZeroArgs zr = t_zero_req;
             t_zero_req.P = 0;
             const size_t bsmem = blend_back_smem_bytes(zr.P > 0);
-            LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes(true)));
-            blend_backward_ring_kernel<<<gx * gy, BL_THREADS, bsmem, stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
+            LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes(true)));
+            blend_backward_ring_kernel<false><<<gx * gy, BL_THREADS, bsmem, stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
                                                                                  v->background, img.final_T, img.n_contrib,
                                                                                  dL_dout_color, geo.grad_acc, zr);
             t_rows_zeroed = zr.P > 0;
@@ -2246,7 +2364,25 @@ int lgr_compact_rows(int rows_out, const int32_t* src_row, int n_tensors, const 
 }
 
 // ---- VecTree vector quantisation (row N4) ----
-size_t lgr_vq_workspace_bytes(int64_t n) { return (size_t)(n > 0 ? n : 0) * sizeof(unsigned long long) + 256; }
+// workspace: best[n] (64-bit score | code) followed by the deterministic mode's sort buffers (codes and sample rows, in and out) and the
+// radix sort's temporary storage; the size does not depend on the mode, so a workspace stays valid when the mode changes
+struct VqDetLayout { size_t codes_in, codes_out, rows_in, rows_out, temp, temp_bytes, total; };
+VqDetLayout vq_det_layout(int64_t n)
+{
+    VqDetLayout L;
+    const size_t m = (size_t)(n > 0 ? n : 0);
+    L.codes_in = align_up(m * sizeof(unsigned long long), 256);
+    L.codes_out = L.codes_in + align_up(m * 4, 256);
+    L.rows_in = L.codes_out + align_up(m * 4, 256);
+    L.rows_out = L.rows_in + align_up(m * 4, 256);
+    L.temp = L.rows_out + align_up(m * 4, 256);
+    L.temp_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, L.temp_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
+                                    (uint32_t*)nullptr, (int)(m ? m : 1), 0, 32);
+    L.total = L.temp + align_up(L.temp_bytes, 256) + 256;
+    return L;
+}
+size_t lgr_vq_workspace_bytes(int64_t n) { return vq_det_layout(n).total; }
 
 int lgr_vq_assign(int n, int d, int K, const float* x, const float* embed, const float* weight, const float* weight_sum, int32_t* idx,
                   float* cluster_batch, float* embed_sum, void* workspace, void* cuda_stream)
@@ -2315,6 +2451,28 @@ int lgr_vq_assign(int n, int d, int K, const float* x, const float* embed, const
         else if (d <= 48) vq_launch_assign<48>(n, d, K, x, embed, best, stream);
         else vq_launch_assign<64>(n, d, K, x, embed, best, stream);
         LGR_LAUNCH_CHECK("vq_assign_kernel", false, stream);
+    }
+    if (g_det) {
+        // deterministic mode: stable sort of (code, sample) pairs on log2(K) bits, then per-code sums in ascending sample order
+        const VqDetLayout L = vq_det_layout(n);
+        char* ws = static_cast<char*>(workspace);
+        uint32_t* codes_in = reinterpret_cast<uint32_t*>(ws + L.codes_in);
+        uint32_t* codes_out = reinterpret_cast<uint32_t*>(ws + L.codes_out);
+        uint32_t* rows_in = reinterpret_cast<uint32_t*>(ws + L.rows_in);
+        uint32_t* rows_out = reinterpret_cast<uint32_t*>(ws + L.rows_out);
+        int bits = 1;
+        while ((1ll << bits) < (long long)K) bits++;
+        ProfScope ps(ST_VQ_ASSIGN, stream);
+        vq_det_keys_kernel<<<(n + 255) / 256, 256, 0, stream>>>(n, best, idx, codes_in, rows_in);
+        LGR_LAUNCH_CHECK("vq_det_keys_kernel", false, stream);
+        if (cluster_batch || embed_sum) {
+            size_t tmp = L.temp_bytes;
+            LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(ws + L.temp, tmp, codes_in, codes_out, rows_in, rows_out, n, 0, bits, stream));
+            vq_det_segsum_kernel<<<(unsigned)K, VQ_SEG_WARPS * 32, 0, stream>>>(n, d, K, codes_out, rows_out, x, weight, (float)n, weight_sum,
+                                                                                         cluster_batch, embed_sum);
+            LGR_LAUNCH_CHECK("vq_det_segsum_kernel", false, stream);
+        }
+        return LGR_OK;
     }
     const long long total = (long long)n * (d + 1);
     vq_accumulate_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(n, d, best, x, weight, (float)n, weight_sum, idx, cluster_batch,

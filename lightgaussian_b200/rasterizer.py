@@ -41,11 +41,21 @@ class GaussianRasterizationSettings(NamedTuple):
 
 
 _last_R = [0]
+_last_deterministic = [False]
 
 
 def last_num_rendered() -> int:
     """num_rendered of the most recent forward call in this process (diagnostics / bench.py)."""
     return _last_R[0]
+
+
+def _apply_deterministic_mode() -> bool:
+    """Deterministic mode of a forward, decided at the time of the call (capi.deterministic_requested) and set in the library.
+    The autograd nodes record it, and their backward runs in that mode whatever the flag says by then."""
+    det = capi.deterministic_requested()
+    capi.set_deterministic(det)
+    _last_deterministic[0] = det
+    return det
 
 
 def _f32c(t, name):
@@ -89,6 +99,7 @@ def _forward_native(count_mode, background, means3D, colors, opacity, scales, ro
     if count_mode:
         count = torch.empty((P,), dtype=torch.int32, device=device)
         score = torch.empty((P,), dtype=torch.float32, device=device)
+    _apply_deterministic_mode()
     slots = [capi.BlobSlot(device) for _ in range(3)]
     num_rendered = C.c_int32(0)
     try:
@@ -192,6 +203,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = _C.rasterize_gaussians(*args)
         ctx.raster_settings = raster_settings
         ctx.num_rendered = num_rendered
+        ctx.deterministic = _last_deterministic[0]
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer)
         ctx.mark_non_differentiable(radii)
         return color, radii
@@ -200,6 +212,7 @@ class _RasterizeGaussians(torch.autograd.Function):
     def backward(ctx, grad_out_color, _):
         rs = ctx.raster_settings
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
+        capi.set_deterministic(ctx.deterministic)   # the mode of the forward, whatever the flag says now
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
          grad_rotations) = _C.rasterize_gaussians_backward(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
@@ -315,6 +328,7 @@ def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacit
     if count_mode:
         count = torch.empty((P,), dtype=torch.int32, device=device)
         score = torch.empty((P,), dtype=torch.float32, device=device)
+    _apply_deterministic_mode()
     slots = [capi.BlobSlot(device) for _ in range(3)]
     num_rendered = C.c_int32(0)
     try:
@@ -357,6 +371,7 @@ def forward_vq_native(count_mode, rs, xyz, store):
     params = capi.LgrVqResidentParams(capi.ptr(xyz), capi.ptr(store.attr), capi.ptr(store.slot), capi.ptr(store.codebook),
                                       capi.ptr(store.nonvq), int(store.attr.dtype == torch.float16),
                                       int(store.nonvq.dtype == torch.float16), store.D, store.Dp, store.K)
+    _apply_deterministic_mode()
     slots = [capi.BlobSlot(device) for _ in range(3)]
     num_rendered = C.c_int32(0)
     try:
@@ -421,6 +436,7 @@ class _RasterizeRawLeaves(torch.autograd.Function):
         _, _, R, color, radii, geom, binning, img, leaves = _forward_raw_native(False, raster_settings, xyz, dc, rest, scaling, rotation, opacity)
         ctx.raster_settings = raster_settings
         ctx.num_rendered = R
+        ctx.deterministic = _last_deterministic[0]
         ctx.save_for_backward(*leaves, radii, geom, binning, img)
         ctx.mark_non_differentiable(radii)
         return color, radii
@@ -429,6 +445,7 @@ class _RasterizeRawLeaves(torch.autograd.Function):
     def backward(ctx, grad_out_color, _):
         rs = ctx.raster_settings
         xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img = ctx.saved_tensors
+        capi.set_deterministic(ctx.deterministic)   # the mode of the forward, whatever the flag says now
         world = _exchange["world"]
         exchange = world > 1 and xyz.size(0) != 0 and rest.size(1) > 0
         sparse_single = world == 1 and _os.environ.get("LGR_SPARSE_SINGLE", "0") == "1" and xyz.size(0) != 0 and rest.size(1) > 0

@@ -52,6 +52,7 @@ def vq_assign(x, embed, weight=None, want_sums=False):
         if weight.shape[0] != n:
             raise RuntimeError("vq_assign: one weight per sample expected")
         wsum = weight.sum()
+    capi.set_deterministic(capi.deterministic_requested())   # the rasterizer's rule, at the time of the call
     with torch.cuda.device(dev):
         st = lib.lgr_vq_assign(n, d, K, capi.ptr(x), embed.data_ptr(), capi.ptr(weight), capi.ptr(wsum), capi.ptr(idx), capi.ptr(cb), capi.ptr(es),
                                ws.data_ptr(), capi.current_stream_ptr(dev))
