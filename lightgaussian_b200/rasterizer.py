@@ -561,6 +561,22 @@ def _symm_exchange(device, P, world, group):
     return _symm_cache[key]
 
 
+def _exchange_tables(bases, rank, slot_bytes, push):
+    """The pointer tables of one rank of the sparse exchange, per buffer k (bases[k][q] = address of rank q's buffer k, as mapped on
+    this rank): (pack_tables, ptr_tables) -- where this rank's packed view goes, and where the accumulate kernel reads view v.
+      push: slot `rank` of every rank's buffer; view v is read from slot v of this rank's own buffer.
+      pull: slot `rank` of this rank's own buffer only; view v is read from slot v of rank v's buffer."""
+    world = len(bases[0])
+    r = rank
+    if push:
+        pack = [(C.c_void_p * world)(*[t[q] + r * slot_bytes for q in range(world)]) for t in bases]
+        ptrs = [(C.c_void_p * world)(*[t[r] + v * slot_bytes for v in range(world)]) for t in bases]
+    else:
+        pack = [(C.c_void_p * 1)(t[r] + r * slot_bytes) for t in bases]
+        ptrs = [(C.c_void_p * world)(*[t[v] + v * slot_bytes for v in range(world)]) for t in bases]
+    return pack, ptrs
+
+
 class _SparseExchange:
     """Two alternating exchange buffers per rank in NVLink symmetric memory (torch.distributed._symmetric_memory), each mapped into every
     peer, for the sparse gradient exchange (csrc/lgr_sparse.cuh).  A buffer holds `world` slots; slot v carries view v's packed gradient
@@ -600,14 +616,7 @@ class _SparseExchange:
             b.zero_()
         for t in bases:
             assert len(t) == world and all(t) and all(p % 256 == 0 for p in t)
-        r = self.rank
-        # pack: where this rank's view goes.  accumulate: where view v is read from.
-        if self.push:
-            self.pack_tables = [(C.c_void_p * world)(*[t[q] + r * slot for q in range(world)]) for t in bases]
-            self.ptr_tables = [(C.c_void_p * world)(*[t[r] + v * slot for v in range(world)]) for t in bases]
-        else:
-            self.pack_tables = [(C.c_void_p * 1)(t[r] + r * slot) for t in bases]
-            self.ptr_tables = [(C.c_void_p * world)(*[t[v] + v * slot for v in range(world)]) for t in bases]
+        self.pack_tables, self.ptr_tables = _exchange_tables(bases, self.rank, slot, self.push)
         self.slot_bytes = slot
         self.turn = 0
 
@@ -670,33 +679,49 @@ def _backward_raw_sparse(xs, rs, num_rendered, grad_out_color, xyz, dc, rest, sc
     """View-parallel backward with the sparse exchange: blend backward | flag + scan + per-Gaussian backward of the ~13 % of Gaussians with a
     non-zero gradient, published in peer-mapped memory | one cross-GPU barrier | every rank reads all views' rows over NVLink and writes the
     dense, summed leaf gradients (bit-identical on every rank).  No NCCL call, no host synchronisation."""
+    device = xyz.device
+    P = xyz.size(0)
+    g2d = torch.empty((P, 3), dtype=torch.float32, device=device)
+    g = [torch.empty(t.shape, dtype=torch.float32, device=device) for t in (xyz, dc, rest, scaling, rotation, opacity)]
+    k = xs.next()
+    with torch.cuda.device(device):
+        _sparse_pack(xs, k, rs, num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img, g2d)
+        if world > 1:
+            xs.hdls[k].barrier(channel=0)          # every rank's rows of this step are published
+        _sparse_accumulate(xs, k, int(rs.sh_degree), world, xyz, rest, g)
+    return g, g2d
+
+
+def _sparse_pack(xs, k, rs, num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img, g2d):
+    """First half of the sparse backward, on the current stream of xyz's device: blend backward, then flag + scan + per-Gaussian backward
+    of the flagged Gaussians into this rank's slot of exchange buffer k (every rank's, in push mode).  Writes this view's dL/dmeans2D
+    into g2d [P,3]."""
     lib = capi.load()
     device = xyz.device
     P, M = xyz.size(0), 1 + rest.size(1)
     H, W = grad_out_color.size(1), grad_out_color.size(2)
-    g2d = torch.empty((P, 3), dtype=torch.float32, device=device)
-    g = [torch.empty(t.shape, dtype=torch.float32, device=device) for t in (xyz, dc, rest, scaling, rotation, opacity)]
     dpix = _f32c(grad_out_color, "grad_out_color")
-    main = torch.cuda.current_stream(device)
-    k = xs.next()
-    with torch.cuda.device(device):
-        view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W, rs.scale_modifier,
-                                rs.sh_degree, False, rs.debug)
-        st = lib.lgr_backward_raw_begin(C.byref(view), P, int(num_rendered), radii.data_ptr(), geom.data_ptr(), binning.data_ptr(),
-                                        img.data_ptr(), dpix.data_ptr(), None, main.cuda_stream)
-        capi.check(st, "lgr_backward_raw_begin")
-        params = _raw_struct(xyz, dc, rest, scaling, rotation, opacity)
-        st = lib.lgr_backward_raw_sparse_pack_push(C.byref(view), P, M, C.byref(params), radii.data_ptr(), geom.data_ptr(), xs.pack_tables[k],
-                                                   len(xs.pack_tables[k]), xs.rank if xs.push else 0, xs.ws.data_ptr(), g2d.data_ptr(),
-                                                   main.cuda_stream)
-        capi.check(st, "lgr_backward_raw_sparse_pack_push")
-        if world > 1:
-            xs.hdls[k].barrier(channel=0)          # every rank's rows of this step are published
-        grads = _raw_grads_struct(*g)
-        st = lib.lgr_backward_raw_sparse_accumulate(P, M, int(rs.sh_degree), world, xs.ptr_tables[k], xyz.data_ptr(), C.byref(grads),
-                                                    main.cuda_stream)
-        capi.check(st, "lgr_backward_raw_sparse_accumulate")
-    return g, g2d
+    stream = capi.current_stream_ptr(device)
+    view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W, rs.scale_modifier,
+                            rs.sh_degree, False, rs.debug)
+    st = lib.lgr_backward_raw_begin(C.byref(view), P, int(num_rendered), radii.data_ptr(), geom.data_ptr(), binning.data_ptr(),
+                                    img.data_ptr(), dpix.data_ptr(), None, stream)
+    capi.check(st, "lgr_backward_raw_begin")
+    params = _raw_struct(xyz, dc, rest, scaling, rotation, opacity)
+    st = lib.lgr_backward_raw_sparse_pack_push(C.byref(view), P, M, C.byref(params), radii.data_ptr(), geom.data_ptr(), xs.pack_tables[k],
+                                               len(xs.pack_tables[k]), xs.rank if xs.push else 0, xs.ws.data_ptr(), g2d.data_ptr(), stream)
+    capi.check(st, "lgr_backward_raw_sparse_pack_push")
+
+
+def _sparse_accumulate(xs, k, sh_degree, world, xyz, rest, g):
+    """Second half, once every rank's view is in buffer k: the six dense leaf gradients g (list of [P,...] float32 tensors), summed
+    over the `world` views in rank order."""
+    lib = capi.load()
+    P, M = xyz.size(0), 1 + rest.size(1)
+    grads = _raw_grads_struct(*g)
+    st = lib.lgr_backward_raw_sparse_accumulate(P, M, int(sh_degree), world, xs.ptr_tables[k], xyz.data_ptr(), C.byref(grads),
+                                                capi.current_stream_ptr(xyz.device))
+    capi.check(st, "lgr_backward_raw_sparse_accumulate")
 
 
 def _exchange_chunks(P):
