@@ -20,7 +20,8 @@
 //         dL/dcolor[c] = sum_l w[l] * dpix_c[l]          S_k = sum_l wg[l] * {1, x_l, y_l, x_l^2, x_l y_l, y_l^2}
 //     so a pair parks TWO floats per lane (was nine), and every 16 pairs the warp contracts the 16x32 tables against the coefficient
 //     table in shared memory -- lane p owns pair p, half-warps split the 32 source lanes, immediates for the offsets -- converts the
-//     moments from sub-tile-origin to Gaussian-centred form and issues the atomics.  ~14 instructions per pair instead of ~45.
+//     moments from sub-tile-origin to Gaussian-centred form and adds the nine sums to the record with two 16-byte vector reductions
+//     and one scalar reduction (three L2 atomic operations per pair, not nine).  ~14 instructions per pair instead of ~45.
 //   * backward: exp through ex2.approx on log2(e)*power (1e-3 contract), non-contributing lanes are folded in as alpha = 0
 //     (neutral for T, the colour recurrence and every sum), so the pair body is branch-free.
 #pragma once
@@ -51,6 +52,12 @@ __device__ __forceinline__ void mbar_wait_ring(uint64_t* bar, uint32_t parity)
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// four float atomic adds to consecutive words as ONE vector reduction (sm_90, SASS REDG.E.ADD.F32x4): one L2 operation instead of four.
+// `addr` must be 16-byte aligned.  Like atomicAdd on f32, it flushes subnormals to zero.
+__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d)
+{
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
 
 // sub-tile cull with a magnitude-aware margin: the 1 % alpha margin covers the rounding of q only while its terms stay below ~1e4;
 // an elongated splat far from the rectangle can cancel terms of 1e6-1e7 down to a small q, so the rounding bound of the evaluated
@@ -383,17 +390,14 @@ __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, in
             row[5] = s1y; row[6] = s2xx; row[7] = s2xy; row[8] = s2yy;
         }
     } else if (p < nbuf) {
+        // both halves hold all nine sums: lane p adds words 0-3 of the record, lane p + 16 words 4-7 and word 8.  Records are 48 bytes
+        // and grad_acc is 256-byte aligned (a 256-byte offset in carve_geometry of a blob lgr_alloc_fn returns 256-byte aligned), so rec
+        // and rec + 4 are 16-byte aligned.
         float* rec = acc + (size_t)__float_as_uint(bw.mid[p]) * ACC_STRIDE;
         if (h == 0) {
-            atomicAdd(rec + 0, c0);
-            atomicAdd(rec + 1, c1);
-            atomicAdd(rec + 2, c2);
-            atomicAdd(rec + 3, s0);
-            atomicAdd(rec + 4, s1x);
+            red_add_v4(rec, c0, c1, c2, s0);
         } else {
-            atomicAdd(rec + 5, s1y);
-            atomicAdd(rec + 6, s2xx);
-            atomicAdd(rec + 7, s2xy);
+            red_add_v4(rec + 4, s1x, s1y, s2xx, s2xy);
             atomicAdd(rec + 8, s2yy);
         }
     }
