@@ -233,6 +233,30 @@ int lgr_backward_raw_sparse_pack(const lgr_view* v, int P, int M, const lgr_raw_
 int lgr_backward_raw_sparse_accumulate(int P, int M, int sh_degree, int world, const void* const* peer_buffers, const float* xyz,
                                        const lgr_raw_grads* grads, void* cuda_stream);
 
+/* ---- view-parallel densification statistics (DESIGN.md section 6) ----
+ * lgr_backward_raw_sparse_pack_push_ex: lgr_backward_raw_sparse_pack_push with stats == NULL; with stats, every slot is
+ *   lgr_sparse_exchange_bytes_stats(P) bytes and also carries this view's densification statistics: |dL/dmeans2D[i, 0:2]| in word 14
+ *   of every row, a bitmap of radii > 0 after the rows, and header words 4-6 = 0x53544154, stats->serial, P.
+ * lgr_densify_stats_exchanged: after the barrier of such a step, adds every rank's view in rank order 0..world-1 to accum / denom,
+ *   bit-identical on every rank and to lgr_densify_stats called once per view in that order.  peer_buffers: view v's slot as the
+ *   accumulate kernel reads it.  It also checks the caller's own slot `self` against grad / update_filter (this rank's
+ *   add_densification_stats arguments) and ORs into *error_word: 1 = a slot without statistics, of another serial or another P (those
+ *   32-Gaussian groups are left unchanged), 2 = update_filter != radii > 0, 4 = |grad[i, 0:2]| != the published norm.
+ * lgr_densify_stats_encode / lgr_densify_stats_add_views: the same sum without the sparse exchange.  encode writes one float per
+ *   Gaussian (the norm where update_filter is set, -1.0f elsewhere); add_views adds `world` such rows ([world, P], rank order). */
+typedef struct lgr_sparse_stats {
+    uint32_t serial;
+} lgr_sparse_stats;
+size_t lgr_sparse_exchange_bytes_stats(int P);
+int lgr_backward_raw_sparse_pack_push_ex(const lgr_view* view, int P, int M, const lgr_raw_params* params, const int32_t* radii,
+                                         char* geometry_blob, void* const* slot_of_this_rank, int world, int self, void* workspace,
+                                         float* dL_dmeans2D, const lgr_sparse_stats* stats, void* cuda_stream);
+int lgr_densify_stats_exchanged(int P, int world, int self, const void* const* peer_buffers, uint32_t serial, const float* grad,
+                                int grad_row_stride, const uint8_t* update_filter, float* accum, float* denom, uint32_t* error_word,
+                                void* cuda_stream);
+int lgr_densify_stats_encode(int P, const float* grad, int grad_row_stride, const uint8_t* update_filter, float* out, void* cuda_stream);
+int lgr_densify_stats_add_views(int P, int world, const float* views, float* accum, float* denom, void* cuda_stream);
+
 /* ---- optimizer side of the training loops (SURVEY.md 8f row N3) ----
  * lgr_adamw_step: torch.optim.AdamW's default (foreach) update, amsgrad off, for up to 8 tensors in ONE launch; replaces
  * `gaussians.optimizer.step()` (prune_finetune.py:287, optimizer built at scene/gaussian_model.py:184-217).  `step` is the

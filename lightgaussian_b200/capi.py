@@ -67,6 +67,14 @@ class LgrDensifyTensor(C.Structure):
 DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING, DENSIFY_MOMENT, DENSIFY_ZERO = range(5)   # LGR_DENSIFY_* roles
 
 
+class LgrSparseStats(C.Structure):
+    """struct lgr_sparse_stats"""
+    _fields_ = [("serial", C.c_uint32)]
+
+
+SPARSE_STATS_ERR_HEADER, SPARSE_STATS_ERR_FILTER, SPARSE_STATS_ERR_GRAD = 1, 2, 4   # bits of lgr_densify_stats_exchanged's error word
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 
 _lib = None
@@ -143,6 +151,17 @@ def load():
         lib.lgr_backward_raw_sparse_pack_push.restype = i32
         lib.lgr_backward_raw_sparse_pack_push.argtypes = [C.POINTER(LgrView), i32, i32, C.POINTER(LgrRawParams), vp, vp, C.POINTER(C.c_void_p), i32, i32,
                                                           vp, vp, vp]
+        lib.lgr_sparse_exchange_bytes_stats.restype = C.c_size_t
+        lib.lgr_sparse_exchange_bytes_stats.argtypes = [i32]
+        lib.lgr_backward_raw_sparse_pack_push_ex.restype = i32
+        lib.lgr_backward_raw_sparse_pack_push_ex.argtypes = [C.POINTER(LgrView), i32, i32, C.POINTER(LgrRawParams), vp, vp, C.POINTER(C.c_void_p),
+                                                             i32, i32, vp, vp, C.POINTER(LgrSparseStats), vp]
+        lib.lgr_densify_stats_exchanged.restype = i32
+        lib.lgr_densify_stats_exchanged.argtypes = [i32, i32, i32, C.POINTER(C.c_void_p), C.c_uint32, vp, i32, vp, vp, vp, vp, vp]
+        lib.lgr_densify_stats_encode.restype = i32
+        lib.lgr_densify_stats_encode.argtypes = [i32, vp, i32, vp, vp, vp]
+        lib.lgr_densify_stats_add_views.restype = i32
+        lib.lgr_densify_stats_add_views.argtypes = [i32, i32, vp, vp, vp, vp]
         lib.lgr_backward_raw_sparse_accumulate.restype = i32
         lib.lgr_backward_raw_sparse_accumulate.argtypes = [i32, i32, i32, i32, C.POINTER(C.c_void_p), vp, C.POINTER(LgrRawGrads), vp]
         lib.lgr_vq_workspace_bytes.restype = C.c_size_t

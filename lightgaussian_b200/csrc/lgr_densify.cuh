@@ -31,7 +31,7 @@ namespace {
 constexpr int DEN_MAX_TENSORS = 24;
 constexpr uint8_t DEN_KEEP = 1, DEN_CLONE = 2, DEN_CHILD = 4, DEN_SPLIT = 8;   // class bits of a source row
 
-__device__ __forceinline__ float den_norm2(float a, float b) { return __fsqrt_rn(__fadd_rn(__fmul_rn(a, a), __fmul_rn(b, b))); }
+using lgr::den_norm2;   // lgr_math.cuh: the sparse exchange publishes the same norm
 
 // torch.max(x, dim=1).values of three values: NaN propagates
 __device__ __forceinline__ float den_max3(float a, float b, float c)
@@ -70,6 +70,37 @@ __global__ void __launch_bounds__(256) densify_stats_kernel(int P, const float* 
     const float* g = grad + (long long)i * grad_stride;
     accum[i] = __fadd_rn(accum[i], den_norm2(g[0], g[1]));
     denom[i] = __fadd_rn(denom[i], 1.0f);
+}
+
+// View-parallel statistics when the step's backward did not publish them in the sparse exchange: every rank encodes its view as one
+// float per Gaussian (the norm on the rows of its filter, DEN_NO_VIEW elsewhere: a norm is never negative), the ranks all-gather the
+// rows into [world, P], and densify_stats_views_kernel adds them in rank order with densify_stats_kernel's arithmetic.
+constexpr uint32_t DEN_NO_VIEW = 0xBF800000u;   // -1.0f
+
+__global__ void __launch_bounds__(256) densify_stats_encode_kernel(int P, const float* __restrict__ grad, int grad_stride,
+                                                                   const uint8_t* __restrict__ filter, float* __restrict__ out)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= P) return;
+    const float* g = grad + (long long)i * grad_stride;
+    out[i] = filter[i] ? den_norm2(g[0], g[1]) : __uint_as_float(DEN_NO_VIEW);
+}
+
+__global__ void __launch_bounds__(256) densify_stats_views_kernel(int P, int world, const float* __restrict__ views,
+                                                                  float* __restrict__ accum, float* __restrict__ denom)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= P) return;
+    float acc = accum[i], den = denom[i];
+    bool any = false;
+    for (int v = 0; v < world; v++) {
+        const float x = views[(long long)v * P + i];
+        if (__float_as_uint(x) == DEN_NO_VIEW) continue;
+        acc = __fadd_rn(acc, x);
+        den = __fadd_rn(den, 1.0f);
+        any = true;
+    }
+    if (any) { accum[i] = acc; denom[i] = den; }
 }
 
 struct DensifyPlanArgs {

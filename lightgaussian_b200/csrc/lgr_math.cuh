@@ -461,4 +461,8 @@ LGR_HD void cov3d_backward(float s0, float s1, float s2_, float mod, float r, fl
             4.f * z * (dRm[1][1] + dRm[0][0]);
 }
 
+// torch.norm(g[:, :2], dim=-1) of one row, as torch evaluates it: sqrt(a*a + b*b), each operation rounded on its own.  The densification
+// statistics (lgr_densify.cuh) and the norm the sparse exchange publishes per row (lgr_sparse.cuh) share this one definition.
+LGR_HD float den_norm2(float a, float b) { return LGR_SQRT(LGR_ADD(LGR_MUL(a, a), LGR_MUL(b, b))); }
+
 }  // namespace lgr

@@ -16,14 +16,24 @@
 // basis(dir_v) (x) dRGB_v in registers, and writes every dense output row once.  All ranks add the views in the same order, so the
 // summed gradients are bit-identical on every rank (replicas cannot drift).  Per rank and step the NVLink traffic is
 // (world-1) * (nnz * 64 B + P/4 B) instead of (world-1) * 12 B * P + ~2 * 44 B * P.
+//
+// Densification statistics (view-parallel add_densification_stats, opt-in): the slot then also carries, for free or nearly so,
+//   * word 14 of every row (a zero pad otherwise) = den_norm2(dL/dmeans2D) of the row's Gaussian in this view -- the same bits as the
+//     local dL/dmeans2D the pack writes, and exactly what GaussianModel.add_densification_stats adds for it;
+//   * vis[w32a] after the rows: bit i = radii[i] > 0 in this view (the visibility filter every training loop passes), P/8 bytes;
+//   * header words 4-6: SPX_STATS_MAGIC, the host's step serial, P.
+// densify_stats_exchanged_kernel then adds every rank's view to accum / denom in rank order, bit-identically on every rank.
 #pragma once
 
 namespace {
 
 constexpr int SPX_ROW = 16;  // floats per exchanged row
+constexpr int SPX_NORM = 14; // row word holding the densification norm (stats slots only)
+constexpr uint32_t SPX_STATS_MAGIC = 0x53544154u;   // header word 4 of a slot packed with densification statistics
 
 struct SparseLayout {
     size_t hdr, bitmap, prefix, rows, total;  // offsets in 4-byte words
+    size_t vis, total_stats;                  // visibility bitmap of a stats slot (after the rows), and that slot's size
 };
 __host__ __device__ inline SparseLayout sparse_layout(int P)
 {
@@ -35,30 +45,39 @@ __host__ __device__ inline SparseLayout sparse_layout(int P)
     l.prefix = l.bitmap + w32a;
     l.rows = l.prefix + w32a;
     l.total = l.rows + (size_t)P * SPX_ROW;
+    l.vis = l.total;
+    l.total_stats = l.vis + w32a;
     return l;
 }
 
-// bit i of bitmap = Gaussian i is visible and its blend-backward accumulators are not all zero (=> its gradients may be non-zero)
+// bit i of bitmap = Gaussian i is visible and its blend-backward accumulators are not all zero (=> its gradients may be non-zero);
+// STATS: bit i of vis = Gaussian i is visible
+template <bool STATS>
 __global__ void __launch_bounds__(256) sparse_flag_kernel(int P, const int* __restrict__ radii, const float* __restrict__ acc,
-                                                          uint32_t* __restrict__ bitmap, uint32_t* __restrict__ popc)
+                                                          uint32_t* __restrict__ bitmap, uint32_t* __restrict__ popc, uint32_t* __restrict__ vis)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     bool nz = false;
-    if (i < P && radii[i] > 0) {
+    const bool visible = i < P && radii[i] > 0;
+    if (visible) {
         const float4* r = reinterpret_cast<const float4*>(acc + (size_t)i * ACC_STRIDE);
         const float4 a = r[0], b = r[1];
         const float c = acc[(size_t)i * ACC_STRIDE + 8];
         nz = a.x != 0.f || a.y != 0.f || a.z != 0.f || a.w != 0.f || b.x != 0.f || b.y != 0.f || b.z != 0.f || b.w != 0.f || c != 0.f;
     }
     const unsigned word = __ballot_sync(FULL, nz);
+    unsigned vword = 0;
+    if (STATS) vword = __ballot_sync(FULL, visible);
     if ((threadIdx.x & 31) == 0 && i < P) {
         bitmap[i >> 5] = word;
         popc[i >> 5] = __popc(word);
+        if (STATS) vis[i >> 5] = vword;
     }
 }
 
 __global__ void __launch_bounds__(256) sparse_index_kernel(int P, const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ prefix,
-                                                           int* __restrict__ idx, uint32_t* __restrict__ hdr, const float* __restrict__ campos)
+                                                           int* __restrict__ idx, uint32_t* __restrict__ hdr, const float* __restrict__ campos,
+                                                           int stats, uint32_t serial)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
@@ -68,6 +87,9 @@ __global__ void __launch_bounds__(256) sparse_index_kernel(int P, const uint32_t
     if (i == P - 1) {
         hdr[3] = prefix[i >> 5] + __popc(word);
         hdr[0] = __float_as_uint(campos[0]); hdr[1] = __float_as_uint(campos[1]); hdr[2] = __float_as_uint(campos[2]);
+        if (stats) {
+            hdr[4] = SPX_STATS_MAGIC; hdr[5] = serial; hdr[6] = (uint32_t)P;
+        }
     }
 }
 
@@ -81,11 +103,13 @@ struct SparsePush {
     int n;             // number of destinations (1 = local only)
 };
 
-// header + bitmap + prefix of the local slot -> the peers' slots (small: ~P/4 bytes per peer)
-__global__ void __launch_bounds__(256) sparse_publish_kernel(SparsePush push, int self, size_t words)
+// header + bitmap + prefix of the local slot -> the peers' slots (small: ~P/4 bytes per peer); with statistics also the words
+// [extra_off, extra_off + extra_words) (the visibility bitmap, P/8 bytes)
+__global__ void __launch_bounds__(256) sparse_publish_kernel(SparsePush push, int self, size_t words, size_t extra_off, size_t extra_words)
 {
     const uint32_t* src = push.dst[self];
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (size_t)gridDim.x * blockDim.x) {
+    for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < words + extra_words; j += (size_t)gridDim.x * blockDim.x) {
+        const size_t i = j < words ? j : extra_off + (j - words);
         const uint32_t v = src[i];
         for (int r = 0; r < push.n; r++)
             if (r != self) push.dst[r][i] = v;
@@ -95,6 +119,8 @@ __global__ void __launch_bounds__(256) sparse_publish_kernel(SparsePush push, in
 constexpr int SPK_THREADS = 128;
 constexpr int SPK_ROW = 49;   // floats per staged SH row (48 + 1: conflict-free at one row per lane)
 
+// STATS: word SPX_NORM of every row = den_norm2 of the dL/dmeans2D written for it (a zero pad otherwise)
+template <bool STATS>
 __global__ void __launch_bounds__(SPK_THREADS) preprocess_backward_sparse_kernel(RawBackArgs a, const int* __restrict__ idx, const uint32_t* __restrict__ hdr,
                                                                                  SparsePush push, size_t rows_off)
 {
@@ -175,7 +201,7 @@ __global__ void __launch_bounds__(SPK_THREADS) preprocess_backward_sparse_kernel
         v0 = make_float4(dRGB[0], dRGB[1], dRGB[2], dmean[0]);
         v1 = make_float4(dmean[1], dmean[2], dscale[0], dscale[1]);
         v2 = make_float4(dscale[2], dq[0], dq[1], dq[2]);
-        v3 = make_float4(dq[3], dop, 0.f, 0.f);
+        v3 = make_float4(dq[3], dop, STATS ? lgr::den_norm2(g2.dm2x, g2.dm2y) : 0.f, 0.f);
         a.dL_dmeans2D[3 * si] = g2.dm2x; a.dL_dmeans2D[3 * si + 1] = g2.dm2y;   // dense [P,3], zero-filled by the caller; local view only
     }
     // The warp's rows are consecutive in every destination slot (row t at t * 64 bytes): they are staged in shared memory (reusing the
@@ -290,6 +316,84 @@ __global__ void __launch_bounds__(256) sparse_accumulate_kernel(SparseAccArgs a)
         for (int k = lane; k < n * nrest; k += 32) a.d_rest[(size_t)first * nrest + k] = s_rest[k];
         for (int k = lane; k < n * 3; k += 32) a.d_dc[(size_t)first * 3 + k] = s_dc[k];
     }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// View-parallel add_densification_stats from the step's stats slots.  One thread per Gaussian, lane v of a warp fetches view v's bitmap
+// word, prefix, visibility word and header; every thread walks the views 0..world-1 in order and, where view v saw its Gaussian, adds
+// word SPX_NORM of its row (flagged) or +0.0f (visible with no row: its dL/dmeans2D is zero, so the serial call adds den_norm2(0, 0) = +0)
+// to accum and 1 to denom -- the arithmetic of densify_stats_kernel called once per view in rank order.
+// The same pass checks the caller against its own slot and ORs into *err:
+//   SPX_ERR_HEADER  a slot without statistics, from another step (serial) or for another P: the warp adds nothing (its prefix words
+//                   cannot be trusted to address rows)
+//   SPX_ERR_FILTER  update_filter[i] != the published radii[i] > 0
+//   SPX_ERR_GRAD    den_norm2(grad[i, 0:2]) != the published norm (0 for a visible row without one)
+// ------------------------------------------------------------------------------------------------------------------
+constexpr uint32_t SPX_ERR_HEADER = 1u, SPX_ERR_FILTER = 2u, SPX_ERR_GRAD = 4u;
+
+struct DensifyExchArgs {
+    int P, world, self;
+    uint32_t serial;
+    const uint32_t* slot[8];   // view v's slot, as the accumulate kernel reads it
+    const float* grad;         // this rank's dL/dmeans2D rows
+    int grad_stride;
+    const uint8_t* filter;     // this rank's update filter
+    float* accum;
+    float* denom;
+    uint32_t* err;
+};
+
+__global__ void __launch_bounds__(256) densify_stats_exchanged_kernel(DensifyExchArgs a)
+{
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int first = blockIdx.x * 256 + warp * 32;
+    if (first >= a.P) return;
+    const int i = first + lane;
+    const bool in = i < a.P;
+    const SparseLayout L = sparse_layout(a.P);
+    uint32_t my_word = 0, my_pre = 0, my_vis = 0;
+    unsigned long long my_base = 0;
+    bool bad = false;
+    if (lane < a.world) {
+        const uint32_t* base = a.slot[lane];
+        my_base = reinterpret_cast<unsigned long long>(base);
+        bad = base[L.hdr + 4] != SPX_STATS_MAGIC || base[L.hdr + 5] != a.serial || base[L.hdr + 6] != (uint32_t)a.P;
+        if (!bad) {
+            my_word = base[L.bitmap + (first >> 5)];
+            my_pre = base[L.prefix + (first >> 5)];
+            my_vis = base[L.vis + (first >> 5)];
+        }
+    }
+    if (__any_sync(FULL, bad)) {
+        if (lane == 0) atomicOr(a.err, SPX_ERR_HEADER);
+        return;
+    }
+    uint32_t err = 0;
+    float acc = 0.f, den = 0.f;
+    if (in) { acc = a.accum[i]; den = a.denom[i]; }
+    const unsigned below = (1u << lane) - 1u;
+    for (int v = 0; v < a.world; v++) {
+        const uint32_t word = __shfl_sync(FULL, my_word, v);
+        const uint32_t pre = __shfl_sync(FULL, my_pre, v);
+        const uint32_t vis = __shfl_sync(FULL, my_vis, v);
+        const uint32_t* base = reinterpret_cast<const uint32_t*>(__shfl_sync(FULL, my_base, v));
+        if (!in) continue;
+        const bool visible = (vis >> lane) & 1u, flagged = (word >> lane) & 1u;
+        float nrm = 0.f;
+        if (flagged) nrm = __uint_as_float(base[L.rows + ((size_t)pre + __popc(word & below)) * SPX_ROW + SPX_NORM]);
+        if (visible) {
+            acc = __fadd_rn(acc, nrm);
+            den = __fadd_rn(den, 1.0f);
+        }
+        if (v == a.self) {
+            if ((a.filter[i] != 0) != visible) err |= SPX_ERR_FILTER;
+            const float* g = a.grad + (size_t)i * a.grad_stride;
+            if (visible && __float_as_uint(lgr::den_norm2(g[0], g[1])) != __float_as_uint(nrm)) err |= SPX_ERR_GRAD;
+        }
+    }
+    if (in) { a.accum[i] = acc; a.denom[i] = den; }
+    err = __reduce_or_sync(FULL, err);
+    if (lane == 0 && err) atomicOr(a.err, err);
 }
 
 // ------------------------------------------------------------------------------------------------------------------

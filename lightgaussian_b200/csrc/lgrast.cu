@@ -2002,6 +2002,17 @@ int lgr_backward_raw_sparse_pack_push(const lgr_view* v, int P, int M, const lgr
                                       void* const* slot_of_this_rank, int world, int self, void* workspace, float* dL_dmeans2D,
                                       void* cuda_stream)
 {
+    return lgr_backward_raw_sparse_pack_push_ex(v, P, M, params, radii, geometry_blob, slot_of_this_rank, world, self, workspace, dL_dmeans2D,
+                                                nullptr, cuda_stream);
+}
+
+size_t lgr_sparse_exchange_bytes_stats(int P) { return P > 0 ? sparse_layout(P).total_stats * 4 : 256; }
+
+// stats != NULL: the slots are lgr_sparse_exchange_bytes_stats(P) bytes and also carry the densification statistics (lgr_sparse.cuh)
+int lgr_backward_raw_sparse_pack_push_ex(const lgr_view* v, int P, int M, const lgr_raw_params* params, const int32_t* radii, char* geometry_blob,
+                                         void* const* slot_of_this_rank, int world, int self, void* workspace, float* dL_dmeans2D,
+                                         const lgr_sparse_stats* stats, void* cuda_stream)
+{
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     if (P == 0) return LGR_OK;
     if (!v || P < 0 || M < 1 || !params || !radii || !geometry_blob || !slot_of_this_rank || world < 1 || world > 8 || self < 0 || self >= world ||
@@ -2049,11 +2060,19 @@ int lgr_backward_raw_sparse_pack_push(const lgr_view* v, int P, int M, const lgr
     {
         ProfScope ps(ST_SPARSE_PACK, stream);
         LGR_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D, 0, sizeof(float) * 3 * (size_t)P, stream));
-        sparse_flag_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, radii, geo.grad_acc, xb + L.bitmap, popc);
+        if (stats)
+            sparse_flag_kernel<true><<<(P + 255) / 256, 256, 0, stream>>>(P, radii, geo.grad_acc, xb + L.bitmap, popc, xb + L.vis);
+        else
+            sparse_flag_kernel<false><<<(P + 255) / 256, 256, 0, stream>>>(P, radii, geo.grad_acc, xb + L.bitmap, popc, nullptr);
         LGR_CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, popc, xb + L.prefix, w32, stream));
-        sparse_index_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, xb + L.bitmap, xb + L.prefix, idx, xb + L.hdr, v->campos);
-        if (world > 1) sparse_publish_kernel<<<LGR_SMS, 256, 0, stream>>>(push, self, L.rows);
-        preprocess_backward_sparse_kernel<<<(P + SPK_THREADS - 1) / SPK_THREADS, SPK_THREADS, 0, stream>>>(a, idx, xb + L.hdr, push, L.rows);
+        sparse_index_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, xb + L.bitmap, xb + L.prefix, idx, xb + L.hdr, v->campos, stats ? 1 : 0,
+                                                                 stats ? stats->serial : 0u);
+        if (world > 1)
+            sparse_publish_kernel<<<LGR_SMS, 256, 0, stream>>>(push, self, L.rows, L.vis, stats ? L.total_stats - L.vis : 0);
+        if (stats)
+            preprocess_backward_sparse_kernel<true><<<(P + SPK_THREADS - 1) / SPK_THREADS, SPK_THREADS, 0, stream>>>(a, idx, xb + L.hdr, push, L.rows);
+        else
+            preprocess_backward_sparse_kernel<false><<<(P + SPK_THREADS - 1) / SPK_THREADS, SPK_THREADS, 0, stream>>>(a, idx, xb + L.hdr, push, L.rows);
     }
     LGR_LAUNCH_CHECK("preprocess_backward_sparse_kernel", debug, stream);
     return LGR_OK;
@@ -2090,6 +2109,33 @@ int lgr_backward_raw_sparse_accumulate(int P, int M, int sh_degree, int world, c
         sparse_accumulate_kernel<<<(P + 255) / 256, 256, smem, stream>>>(a);
     }
     LGR_LAUNCH_CHECK("sparse_accumulate_kernel", false, stream);
+    return LGR_OK;
+}
+
+int lgr_densify_stats_exchanged(int P, int world, int self, const void* const* peer_buffers, uint32_t serial, const float* grad,
+                                int grad_row_stride, const uint8_t* update_filter, float* accum, float* denom, uint32_t* error_word,
+                                void* cuda_stream)
+{
+    if (P < 0 || world < 1 || world > 8 || self < 0 || self >= world || grad_row_stride < 2 || !peer_buffers ||
+        (P && (!grad || !update_filter || !accum || !denom || !error_word))) {
+        g_last_error = "lgr_densify_stats_exchanged: bad argument (1..8 ranks, 0 <= self < world, grad_row_stride >= 2, all pointers set)";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P == 0) return LGR_OK;
+    DensifyExchArgs a;
+    memset(&a, 0, sizeof(a));
+    a.P = P; a.world = world; a.self = self; a.serial = serial;
+    for (int r = 0; r < world; r++) {
+        if (!peer_buffers[r] || ((uintptr_t)peer_buffers[r] & 255)) {
+            g_last_error = "lgr_densify_stats_exchanged: peer buffer missing or not 256-byte aligned";
+            return LGR_ERR_INVALID_ARG;
+        }
+        a.slot[r] = static_cast<const uint32_t*>(peer_buffers[r]);
+    }
+    a.grad = grad; a.grad_stride = grad_row_stride; a.filter = update_filter; a.accum = accum; a.denom = denom; a.err = error_word;
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    densify_stats_exchanged_kernel<<<(P + 255) / 256, 256, 0, stream>>>(a);
+    LGR_LAUNCH_CHECK("densify_stats_exchanged_kernel", false, stream);
     return LGR_OK;
 }
 
@@ -2634,6 +2680,32 @@ int lgr_densify_stats(int P, const float* grad, int grad_row_stride, const uint8
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     densify_stats_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, grad, grad_row_stride, update_filter, accum, denom);
     LGR_LAUNCH_CHECK("densify_stats_kernel", false, stream);
+    return LGR_OK;
+}
+
+int lgr_densify_stats_encode(int P, const float* grad, int grad_row_stride, const uint8_t* update_filter, float* out, void* cuda_stream)
+{
+    if (P < 0 || grad_row_stride < 2 || (P && (!grad || !update_filter || !out))) {
+        g_last_error = "lgr_densify_stats_encode: bad argument (P >= 0, grad_row_stride >= 2, all pointers set)";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P == 0) return LGR_OK;
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    densify_stats_encode_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, grad, grad_row_stride, update_filter, out);
+    LGR_LAUNCH_CHECK("densify_stats_encode_kernel", false, stream);
+    return LGR_OK;
+}
+
+int lgr_densify_stats_add_views(int P, int world, const float* views, float* accum, float* denom, void* cuda_stream)
+{
+    if (P < 0 || world < 1 || (P && (!views || !accum || !denom))) {
+        g_last_error = "lgr_densify_stats_add_views: bad argument (P >= 0, world >= 1, all pointers set)";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P == 0) return LGR_OK;
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    densify_stats_views_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, world, views, accum, denom);
+    LGR_LAUNCH_CHECK("densify_stats_views_kernel", false, stream);
     return LGR_OK;
 }
 

@@ -18,7 +18,7 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import capi, trace
+from . import capi, rasterizer, trace
 from .optim import _GROUP_ATTR
 
 _ROLE = {"xyz": capi.DENSIFY_XYZ, "scaling": capi.DENSIFY_SCALING}
@@ -45,22 +45,128 @@ def _dense_f32(t, device, shape) -> bool:
 
 
 def add_densification_stats(gaussians, viewspace_point_tensor, update_filter):
-    """GaussianModel.add_densification_stats (:784-788)"""
+    """GaussianModel.add_densification_stats (:784-788).  With the view-parallel densification exchange on
+    (parallel.enable_gradient_exchange(world > 1, densification=True)) it adds every rank's view of the step, in rank order, on every
+    rank: from the slots of the step's sparse exchange when its backward published them, else through one all-gather."""
     grad = getattr(viewspace_point_tensor, "grad", None)
     accum, denom = getattr(gaussians, "xyz_gradient_accum", None), getattr(gaussians, "denom", None)
     P = accum.shape[0] if isinstance(accum, torch.Tensor) else -1
     device = grad.device if isinstance(grad, torch.Tensor) else None
+    exchanged = rasterizer.densification_exchange()
     if not (isinstance(grad, torch.Tensor) and grad.is_cuda and grad.dtype == torch.float32 and grad.dim() == 2 and grad.shape[0] == P
             and grad.shape[1] >= 2 and grad.stride(1) == 1 and grad.stride(0) >= 2
             and isinstance(update_filter, torch.Tensor) and update_filter.dtype == torch.bool and update_filter.device == device
             and update_filter.is_contiguous() and tuple(update_filter.shape) == (P,)
             and _dense_f32(accum, device, (P, 1)) and _dense_f32(denom, device, (P, 1))):
+        if exchanged:   # the class's own method would add this rank's view only: the replicas would take different decisions
+            raise RuntimeError("view-parallel densification needs a float32 CUDA view-space gradient [P,>=2], a contiguous bool filter [P] "
+                               "and float32 [P,1] xyz_gradient_accum / denom on the same device")
         return _original(gaussians, "add_densification_stats")(gaussians, viewspace_point_tensor, update_filter)
+    if exchanged:
+        ex = rasterizer._exchange
+        rec, ex["stats_record"] = ex["stats_record"], None
+        if rec is not None and rec["P"] == P and rec["device"] == device:
+            xs = rec["xs"]
+            stats_exchanged(xs, rec["k"], xs.rank, rec["serial"], ex["world"], grad, update_filter, accum, denom)
+        else:
+            stats_allgather(grad, update_filter, accum, denom, ex["world"], ex["group"])
+        return
     trace.bump("densify_stats_native")
     lib = capi.load()
     with torch.cuda.device(device):
         capi.check(lib.lgr_densify_stats(P, grad.data_ptr(), grad.stride(0), update_filter.data_ptr(), accum.data_ptr(), denom.data_ptr(),
                                          capi.current_stream_ptr(device)), "lgr_densify_stats")
+
+
+_error_words = {}   # "cuda:<index>" -> int32 [1] device word of lgr_densify_stats_exchanged's checks
+
+
+def _device_key(device) -> str:
+    device = torch.device(device)
+    if device.type == "cuda" and device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return str(device)
+
+
+def error_word(device):
+    """the device word the exchanged statistics calls on `device` report mismatches into (see stats_exchanged)"""
+    key = _device_key(device)
+    if key not in _error_words:
+        _error_words[key] = torch.zeros((1,), dtype=torch.int32, device=device)
+    return _error_words[key]
+
+
+def stats_exchanged(xs, k, rank, serial, world, grad, update_filter, accum, denom):
+    """add_densification_stats of a view-parallel step whose backward published its statistics in buffer k of the sparse exchange `xs`
+    (rasterizer._SparseExchange, or one simulated rank of it): every rank's view, in rank order, added to accum / denom.  `rank` is the
+    caller's rank, `serial` the step serial the packs were stamped with.  The kernel checks the caller's own slot against `grad` and
+    `update_filter` and every slot's serial; a mismatch sets error_word(device), which makes the next densify_and_prune raise.
+    No host synchronisation, no collective."""
+    trace.bump("densify_stats_exchanged")
+    lib = capi.load()
+    P, device = accum.shape[0], accum.device
+    err = error_word(device)
+    with torch.cuda.device(device):
+        capi.check(lib.lgr_densify_stats_exchanged(P, int(world), int(rank), xs.ptr_tables[k], int(serial) & 0xFFFFFFFF, grad.data_ptr(),
+                                                   grad.stride(0), update_filter.data_ptr(), accum.data_ptr(), denom.data_ptr(),
+                                                   err.data_ptr(), capi.current_stream_ptr(device)), "lgr_densify_stats_exchanged")
+
+
+def stats_encode(grad, update_filter):
+    """this rank's view as one float32 per Gaussian: |grad[i, :2]| where update_filter is set, -1.0 elsewhere"""
+    lib = capi.load()
+    P, device = update_filter.shape[0], update_filter.device
+    out = torch.empty((P,), dtype=torch.float32, device=device)
+    with torch.cuda.device(device):
+        capi.check(lib.lgr_densify_stats_encode(P, grad.data_ptr(), grad.stride(0), update_filter.data_ptr(), out.data_ptr(),
+                                                capi.current_stream_ptr(device)), "lgr_densify_stats_encode")
+    return out
+
+
+def stats_add_views(views, accum, denom):
+    """adds the encoded views [world, P] to accum / denom in row order, with add_densification_stats' arithmetic"""
+    lib = capi.load()
+    world, P = views.shape
+    device = accum.device
+    views = views.contiguous()
+    with torch.cuda.device(device):
+        capi.check(lib.lgr_densify_stats_add_views(P, world, views.data_ptr(), accum.data_ptr(), denom.data_ptr(),
+                                                   capi.current_stream_ptr(device)), "lgr_densify_stats_add_views")
+
+
+def stats_allgather(grad, update_filter, accum, denom, world, group):
+    """add_densification_stats of a view-parallel step without published statistics (dense exchange, a backward outside the fused
+    node): encode, one all-gather into [world, P] over the exchange group, add the views in rank order"""
+    import torch.distributed as dist
+    trace.bump("densify_stats_allgather")
+    mine = stats_encode(grad, update_filter)
+    views = torch.empty((int(world), mine.shape[0]), dtype=torch.float32, device=mine.device)
+    dist.all_gather_into_tensor(views, mine, group=group)
+    stats_add_views(views, accum, denom)
+
+
+def _exchange_error_to_host(device):
+    """queues the copy of the exchanged statistics' error word into pinned memory and clears the word; None when the exchanged
+    statistics never ran on `device`.  The caller reads the returned tensor after its next stream synchronisation."""
+    word = _error_words.get(_device_key(device))
+    if word is None:
+        return None
+    host = torch.empty((1,), dtype=torch.int32, pin_memory=True)
+    host.copy_(word, non_blocking=True)
+    word.zero_()
+    return host
+
+
+def _raise_on_exchange_error(host):
+    if host is None or int(host[0]) == 0:
+        return
+    e = int(host[0])
+    why = [w for bit, w in ((capi.SPARSE_STATS_ERR_HEADER, "a statistics call that did not match its step's exchange (a pack without "
+                                                             "statistics, another step's buffer, or another P)"),
+                            (capi.SPARSE_STATS_ERR_FILTER, "an update filter other than this view's radii > 0"),
+                            (capi.SPARSE_STATS_ERR_GRAD, "a view-space gradient other than this view's dL/dmeans2D")) if e & bit]
+    raise RuntimeError("view-parallel densification statistics are inconsistent across ranks: " + "; ".join(why) +
+                       ". densify_and_prune refuses to run, so that the replicas cannot diverge")
 
 
 def _groups(gaussians):
@@ -96,6 +202,13 @@ def densify_and_prune(gaussians, max_grad, min_opacity, extent, max_screen_size)
     """GaussianModel.densify_and_prune (:745-761): densify_and_clone, densify_and_split, then the opacity / size prune"""
     groups = _groups(gaussians)
     if groups is None:
+        xyz = getattr(gaussians, "_xyz", None)
+        if isinstance(xyz, torch.Tensor) and xyz.is_cuda:
+            with torch.cuda.device(xyz.device):
+                host = _exchange_error_to_host(xyz.device)
+                if host is not None:
+                    torch.cuda.current_stream(xyz.device).synchronize()
+            _raise_on_exchange_error(host)
         return _original(gaussians, "densify_and_prune")(gaussians, max_grad, min_opacity, extent, max_screen_size)
     trace.bump("densify_native")
     lib = capi.load()
@@ -109,10 +222,15 @@ def densify_and_prune(gaussians, max_grad, min_opacity, extent, max_screen_size)
         stream = capi.current_stream_ptr(device)
         ws = torch.empty((int(lib.lgr_densify_workspace_bytes(P)),), dtype=torch.uint8, device=device)
         counts = (C.c_int32 * 4)()
+        # the checks of the view-parallel statistics calls since the last event: read back with the plan's one synchronisation
+        err_host = _exchange_error_to_host(device)
         capi.check(lib.lgr_densify_plan(P, gaussians.xyz_gradient_accum.data_ptr(), gaussians.denom.data_ptr(), leaf["scaling"].data_ptr(),
                                         leaf["opacity"].data_ptr(), _f32(max_grad), _f32(gaussians.percent_dense * extent), _f32(min_opacity),
                                         _f32(0.1 * extent), int(prune_all), int(bool(max_screen_size)), ws.data_ptr(), ws.numel(), counts,
                                         stream), "lgr_densify_plan")
+        if err_host is not None and P == 0:
+            torch.cuda.current_stream(device).synchronize()   # the plan returns before synchronising when there are no rows
+        _raise_on_exchange_error(err_host)
         kept, clones, children, splits = (int(c) for c in counts)
         # torch.normal(mean=zeros, std) is normal_(0, 1), then mul_(std), add_(mean): the kernel applies n * std + 0.  Drawn even for
         # children pruned later, and when S = 0, as the reference draws them.

@@ -80,13 +80,15 @@ class FlatGrads:
         return self.flat.numel() * 4
 
 
-def enable_gradient_exchange(world: int, group=None):
+def enable_gradient_exchange(world: int, group=None, *, densification: bool = False):
     """Training on `world` ranks: after this call the backward of render()'s fused node returns gradients already summed
     over all ranks' views.  The four small leaves (44 B/Gaussian) go through ONE all-reduce; the SH gradient, which is
     rank-1 per Gaussian and view, is exchanged as its 12 B/Gaussian factor (all-gather) and rebuilt locally
-    (lgr_sh_grad_from_views) -- about 4x less NVLink traffic than all-reducing the dense 12*M B/Gaussian tensor."""
+    (lgr_sh_grad_from_views) -- about 4x less NVLink traffic than all-reducing the dense 12*M B/Gaussian tensor.
+    densification=True: add_densification_stats (the native one, densify.install) adds every rank's view of the step in rank order,
+    so the statistics, and with them every densify_and_prune decision and the model size, stay identical on every rank."""
     from . import rasterizer
-    rasterizer.enable_gradient_exchange(world, group)
+    rasterizer.enable_gradient_exchange(world, group, densification=densification)
 
 
 def allreduce_counts(count: torch.Tensor, world: int) -> torch.Tensor:

@@ -222,6 +222,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         def fit(g, ref):
             return g if ref.numel() != 0 else None
         if _exchange["world"] > 1:
+            _exchange["stats_record"] = None   # no statistics published: add_densification_stats all-gathers them
             # view-parallel training that left the fused node (override_color, convert_SHs_python / compute_cov3D_python, LGR_FUSED=0,
             # a leaf layout the fused kernels cannot read): the replicas must still step on the SUM over all ranks' views, so the
             # per-Gaussian gradients are all-reduced here (dense NCCL: correct, but ~2x slower than the fused sparse exchange).
@@ -393,14 +394,27 @@ def forward_vq_native(count_mode, rs, xyz, store):
 # are already SUMMED over all ranks' views: the dense leaves (xyz, scaling, rotation, opacity: 44 B/Gaussian) go through one
 # all-reduce, while the SH gradient (12*M B/Gaussian) is exchanged as its rank-1 factor dRGB (12 B/Gaussian, all-gather) and
 # rebuilt locally by lgr_sh_grad_from_views -- ~4x less NVLink traffic than all-reducing the dense gradient at degree 3.
-_exchange = {"world": 1, "group": None, "warned_unfused": False, "unfused_calls": 0}
+_exchange = {"world": 1, "group": None, "warned_unfused": False, "unfused_calls": 0,
+             "densify": False,       # view-parallel densification statistics (densify.add_densification_stats)
+             "serial": 0,            # exchanged backwards with statistics so far (the same count on every rank)
+             "stats_record": None}   # what the next statistics call reads: the last exchanged backward's buffer, if it published stats
 
 
-def enable_gradient_exchange(world: int, group=None):
+def enable_gradient_exchange(world: int, group=None, *, densification: bool = False):
     """From now on every rasterizer backward in this process returns per-Gaussian gradients SUMMED over the `world` ranks' views:
     the fused node (`render()` on GaussianModel leaves) through the sparse NVLink peer-memory exchange, every other path through a
-    dense NCCL all-reduce inside `_RasterizeGaussians.backward` -- no path is left that silently keeps rank-local gradients."""
+    dense NCCL all-reduce inside `_RasterizeGaussians.backward` -- no path is left that silently keeps rank-local gradients.
+    densification=True (world > 1): GaussianModel.add_densification_stats (as densify.install makes it) also adds every rank's view of
+    the step, in rank order, so that every rank takes the same densify-and-prune decisions; the sparse exchange then carries the
+    statistics in its slots (DESIGN.md section 6)."""
     _exchange["world"], _exchange["group"] = int(world), group
+    _exchange["densify"] = bool(densification) and int(world) > 1
+    _exchange["stats_record"] = None
+
+
+def densification_exchange() -> bool:
+    """True when add_densification_stats sums every rank's view (enable_gradient_exchange(world > 1, densification=True))"""
+    return _exchange["densify"] and _exchange["world"] > 1
 
 
 def unfused_exchange_calls() -> int:
@@ -449,7 +463,10 @@ class _RasterizeRawLeaves(torch.autograd.Function):
         world = _exchange["world"]
         exchange = world > 1 and xyz.size(0) != 0 and rest.size(1) > 0
         sparse_single = world == 1 and _os.environ.get("LGR_SPARSE_SINGLE", "0") == "1" and xyz.size(0) != 0 and rest.size(1) > 0
-        xs = _sparse_exchange(xyz.device, xyz.size(0), world, _exchange["group"]) if (exchange or sparse_single) else None
+        stats = exchange and _exchange["densify"]
+        xs = _sparse_exchange(xyz.device, xyz.size(0), world, _exchange["group"], stats=stats) if (exchange or sparse_single) else None
+        if world > 1:
+            _exchange["stats_record"] = None   # set again below when this backward publishes statistics
         if xs is not None:
             g, g2d = _backward_raw_sparse(xs, rs, ctx.num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom,
                                           binning, img, world)
@@ -586,16 +603,19 @@ class _SparseExchange:
       pull (LGR_EXCHANGE_PUSH=0, the round-1 scheme): rank r writes slot r of its OWN buffer only; after the barrier the accumulate
                       kernel loads every peer's slot over NVLink.
     Buffer k of step s is rewritten at step s+2; every rank passes the barrier of step s+1 only after its accumulate kernel of step s
-    has finished, so one cross-GPU barrier per step is enough.  world == 1 (tests): plain device tensors, no barrier."""
+    has finished, so one cross-GPU barrier per step is enough.  world == 1 (tests): plain device tensors, no barrier.
+    stats=True: slots of lgr_sparse_exchange_bytes_stats, which also carry each view's densification statistics."""
 
-    def __init__(self, device, P, world, group):
+    def __init__(self, device, P, world, group, stats=False):
         lib = capi.load()
         if world > 8:
             raise RuntimeError("the sparse peer-memory exchange supports at most 8 ranks (one NVSwitch domain)")
         self.world = world
         self.capacity = P          # the layout inside a slot is computed from each call's P <= capacity
+        self.stats = bool(stats)
         self.push = world > 1 and _os.environ.get("LGR_EXCHANGE_PUSH", "1") != "0"
-        slot = (int(lib.lgr_sparse_exchange_bytes(P)) + 255) // 256 * 256
+        nbytes = lib.lgr_sparse_exchange_bytes_stats(P) if self.stats else lib.lgr_sparse_exchange_bytes(P)
+        slot = (int(nbytes) + 255) // 256 * 256
         n = world * slot // 4
         self.ws = torch.empty(int(lib.lgr_sparse_workspace_bytes(P)), dtype=torch.uint8, device=device)
         if world > 1:
@@ -634,25 +654,26 @@ class _SparseExchange:
 _sparse_cache = {}
 
 
-def _sparse_exchange(device, P, world, group):
+def _sparse_exchange(device, P, world, group, stats=False):
     """collectively agreed: either every rank gets the peer-mapped buffers or none does (then the dense NCCL exchange is used).
-    LGR_EXCHANGE=dense selects the dense exchange explicitly."""
+    LGR_EXCHANGE=dense selects the dense exchange explicitly.  stats: slots that carry the densification statistics (every rank asks
+    for the same, enable_gradient_exchange's densification flag)."""
     # ONE exchange object per (device, world), sized for a capacity >= P (kernels lay the buffer out from the call's P): P shrinks at
     # every prune event and may grow when densifying; only growth beyond the capacity re-allocates (x1.25, the old buffers are
     # dropped first), so a training run no longer pins a new pair of peer-mapped buffers per distinct P.
     key = (str(device), world)
     cur = _sparse_cache.get(key, "none")
-    if cur == "none" or (cur is not None and cur.capacity < P):
-        grow = cur != "none" and cur is not None
+    if cur == "none" or (cur is not None and (cur.capacity < P or cur.stats != bool(stats))):
+        grow = cur != "none" and cur is not None and cur.capacity < P
+        cap = max(int(P * 1.25), P) if grow else (P if cur == "none" else max(P, cur.capacity))
         _sparse_cache.pop(key, None)
         del cur
-        cap = int(P * 1.25) if grow else P
         xs, ok = None, 1
         if _os.environ.get("LGR_EXCHANGE", "sparse") != "sparse":
             ok = 0
         else:
             try:
-                xs = _SparseExchange(device, cap, world, group)
+                xs = _SparseExchange(device, cap, world, group, stats=stats)
             except Exception as ex:  # noqa: BLE001  (no P2P / API drift: the NCCL path still works)
                 print(f"lightgaussian_b200: sparse peer-memory exchange unavailable ({type(ex).__name__}: {ex}); using the dense NCCL exchange", flush=True)
                 ok = 0
@@ -684,18 +705,27 @@ def _backward_raw_sparse(xs, rs, num_rendered, grad_out_color, xyz, dc, rest, sc
     g2d = torch.empty((P, 3), dtype=torch.float32, device=device)
     g = [torch.empty(t.shape, dtype=torch.float32, device=device) for t in (xyz, dc, rest, scaling, rotation, opacity)]
     k = xs.next()
+    serial = None
+    if xs.stats:
+        # densification statistics ride in the slots; the statistics call of this step reads buffer k before the next step's barrier
+        _exchange["serial"] = serial = (_exchange["serial"] + 1) & 0xFFFFFFFF
     with torch.cuda.device(device):
-        _sparse_pack(xs, k, rs, num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img, g2d)
+        _sparse_pack(xs, k, rs, num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img, g2d,
+                     serial=serial)
         if world > 1:
             xs.hdls[k].barrier(channel=0)          # every rank's rows of this step are published
         _sparse_accumulate(xs, k, int(rs.sh_degree), world, xyz, rest, g)
+    if serial is not None:
+        _exchange["stats_record"] = dict(xs=xs, k=k, serial=serial, P=P, device=device)
     return g, g2d
 
 
-def _sparse_pack(xs, k, rs, num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img, g2d):
+def _sparse_pack(xs, k, rs, num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img, g2d,
+                 serial=None):
     """First half of the sparse backward, on the current stream of xyz's device: blend backward, then flag + scan + per-Gaussian backward
     of the flagged Gaussians into this rank's slot of exchange buffer k (every rank's, in push mode).  Writes this view's dL/dmeans2D
-    into g2d [P,3]."""
+    into g2d [P,3].  serial (an exchange built with stats=True): the slot also carries this view's densification statistics, stamped
+    with the step serial."""
     lib = capi.load()
     device = xyz.device
     P, M = xyz.size(0), 1 + rest.size(1)
@@ -708,9 +738,16 @@ def _sparse_pack(xs, k, rs, num_rendered, grad_out_color, xyz, dc, rest, scaling
                                     img.data_ptr(), dpix.data_ptr(), None, stream)
     capi.check(st, "lgr_backward_raw_begin")
     params = _raw_struct(xyz, dc, rest, scaling, rotation, opacity)
-    st = lib.lgr_backward_raw_sparse_pack_push(C.byref(view), P, M, C.byref(params), radii.data_ptr(), geom.data_ptr(), xs.pack_tables[k],
-                                               len(xs.pack_tables[k]), xs.rank if xs.push else 0, xs.ws.data_ptr(), g2d.data_ptr(), stream)
-    capi.check(st, "lgr_backward_raw_sparse_pack_push")
+    if serial is None:
+        st = lib.lgr_backward_raw_sparse_pack_push(C.byref(view), P, M, C.byref(params), radii.data_ptr(), geom.data_ptr(), xs.pack_tables[k],
+                                                   len(xs.pack_tables[k]), xs.rank if xs.push else 0, xs.ws.data_ptr(), g2d.data_ptr(), stream)
+        capi.check(st, "lgr_backward_raw_sparse_pack_push")
+        return
+    stats = capi.LgrSparseStats(int(serial) & 0xFFFFFFFF)
+    st = lib.lgr_backward_raw_sparse_pack_push_ex(C.byref(view), P, M, C.byref(params), radii.data_ptr(), geom.data_ptr(), xs.pack_tables[k],
+                                                  len(xs.pack_tables[k]), xs.rank if xs.push else 0, xs.ws.data_ptr(), g2d.data_ptr(),
+                                                  C.byref(stats), stream)
+    capi.check(st, "lgr_backward_raw_sparse_pack_push_ex")
 
 
 def _sparse_accumulate(xs, k, sh_degree, world, xyz, rest, g):
