@@ -305,6 +305,53 @@ LGR_HD float pair_power(float dx, float dy, float A, float B, float Cc)
 }
 
 // ------------------------------------------------------------------------------------------------
+// Exact culling (DESIGN.md section 4): may a rectangle of pixel centres be skipped for a Gaussian?  The offsets dx = px - x and
+// dy = py - y of its pixel centres span [dx_lo, dx_hi] x [dy_lo, dy_hi]; hA = A/2, hC = C/2 and B are the conic's, nba = -B/A,
+// nbc = -B/C.  With the Gaussian's centre outside the rectangle, the smallest q = hA dx^2 + hC dy^2 + B dx dy over it lies on the edge
+// nearest the centre in x or in y; rect_qmin evaluates both candidates (each edge's minimiser clamped to the rectangle) and returns the
+// smaller q with mag, the size of the terms it cancelled.  Returns false when the centre lies inside (q = 0 there).  The operations are
+// pinned: the API path's per-lane mask and the fused path's warp-cooperative mask inline this in different contexts, and must agree bit
+// for bit.
+// ------------------------------------------------------------------------------------------------
+LGR_HD bool rect_qmin(float hA, float hC, float B, float nba, float nbc, float dx_lo, float dx_hi, float dy_lo, float dy_hi, float& q,
+                      float& mag)
+{
+    const float cx = fminf(fmaxf(0.f, dx_lo), dx_hi), cy = fminf(fmaxf(0.f, dy_lo), dy_hi);
+    q = 0.f;
+    mag = 0.f;
+    if (cx == 0.f && cy == 0.f) return false;
+    q = 3.0e38f;
+    if (cx != 0.f) {
+        const float dy = fminf(fmaxf(LGR_MUL(nbc, cx), dy_lo), dy_hi);
+        const float t0 = LGR_MUL(LGR_MUL(hA, cx), cx), t1 = LGR_MUL(LGR_MUL(hC, dy), dy), t2 = LGR_MUL(LGR_MUL(B, cx), dy);
+        q = LGR_ADD(LGR_ADD(t0, t1), t2);
+        mag = LGR_ADD(LGR_MUL(2.f, LGR_ADD(t0, t1)), fabsf(t2));
+    }
+    if (cy != 0.f) {
+        const float dx = fminf(fmaxf(LGR_MUL(nba, cy), dx_lo), dx_hi);
+        const float t0 = LGR_MUL(LGR_MUL(hA, dx), dx), t1 = LGR_MUL(LGR_MUL(hC, cy), cy), t2 = LGR_MUL(LGR_MUL(B, dx), cy);
+        const float qy = LGR_ADD(LGR_ADD(t0, t1), t2);
+        if (qy < q) {
+            q = qy;
+            mag = LGR_ADD(LGR_MUL(2.f, LGR_ADD(t0, t1)), fabsf(t2));
+        }
+    }
+    return true;
+}
+
+// Relative rounding bound of rect_qmin's q and of the reference's own power at a pixel, in units of mag (A dx^2 + C dy^2 + |B dx dy|,
+// the bound lgr_blend.cuh's subtile_cull2 uses).  The 1 % alpha margin in thr = ln(255 * 1.01 * opacity) covers the rounding of q only
+// while its terms stay below ~1e4; a needle far from the rectangle cancels terms of 1e5-1e7 down to a small q.
+#define LGR_CULL_REL 2.0e-6f
+
+// true when no pixel centre of the rectangle can reach alpha >= 1/255 (the reference skips every such pair, forward.cu:345-347).
+LGR_HD bool rect_culled(float hA, float hC, float B, float nba, float nbc, float thr, float dx_lo, float dx_hi, float dy_lo, float dy_hi)
+{
+    float q, mag;
+    return rect_qmin(hA, hC, B, nba, nbc, dx_lo, dx_hi, dy_lo, dy_hi, q, mag) && q > LGR_FMA(LGR_CULL_REL, mag, thr);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Backward per-Gaussian math (RAST/cuda_rasterizer/backward.cu:144-396), free-form float.
 // ------------------------------------------------------------------------------------------------
 struct GradIn {

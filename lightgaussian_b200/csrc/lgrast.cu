@@ -325,28 +325,16 @@ BinningState carve_binning(char* base, size_t R, int W, int H, bool library_binn
 // ------------------------------------------------------------------------------------------------
 // Exact, conservative sub-tile culling.  Returns true when NO pixel centre in [rx0,rx1]x[ry0,ry1] can
 // reach alpha >= 1/255 for this Gaussian, i.e. when the reference would skip every pair at
-// RAST/cuda_rasterizer/forward.cu:345-347.  A 1% margin on alpha covers all rounding in this test.
+// RAST/cuda_rasterizer/forward.cu:345-347.  The margins are lgr::rect_culled's (DESIGN.md section 4).
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool subtile_cull(float gxp, float gyp, float4 co, float rx0, float rx1, float ry0, float ry1)
 {
     const float A = co.x, B = co.y, Cc = co.z;
     const float t = 257.55f * co.w;  // 255 * 1.01 * opacity
     if (t <= 1.0f) return true;      // alpha <= opacity < 1/255 everywhere
-    const float dx_lo = gxp - rx1, dx_hi = gxp - rx0, dy_lo = gyp - ry1, dy_hi = gyp - ry0;
-    const float cx = fminf(fmaxf(0.f, dx_lo), dx_hi), cy = fminf(fmaxf(0.f, dy_lo), dy_hi);
-    if (cx == 0.f && cy == 0.f) return false;                        // centre inside the sub-tile
     if (!(A > 0.f && Cc > 0.f && A * Cc - B * B > 0.f)) return false;  // not positive definite: never cull
-    const float thr = __logf(t);
-    float qmin = 3.0e38f;
-    if (cx != 0.f) {
-        const float dy = fminf(fmaxf(__fdividef(-B * cx, Cc), dy_lo), dy_hi);
-        qmin = 0.5f * (A * cx * cx + Cc * dy * dy) + B * cx * dy;
-    }
-    if (cy != 0.f) {
-        const float dx = fminf(fmaxf(__fdividef(-B * cy, A), dx_lo), dx_hi);
-        qmin = fminf(qmin, 0.5f * (A * dx * dx + Cc * cy * cy) + B * dx * cy);
-    }
-    return qmin > thr;
+    return lgr::rect_culled(0.5f * A, 0.5f * Cc, B, __fdividef(-B, A), __fdividef(-B, Cc), __logf(t), gxp - rx1, gxp - rx0, gyp - ry1,
+                            gyp - ry0);
 }
 
 // Exact tile-level culling at binning time: tile b of a Gaussian's rectangle is dropped when no pixel centre inside
@@ -364,7 +352,7 @@ __device__ __forceinline__ void tile_keep_mask(const lgr::Geom& geo, float4 co, 
     if (area > 64) return;
     if (area < 64) mask = (1ull << area) - 1ull;   // bits >= area stay clear: popcount(mask) = instances listed
     if (!g_tile_cull_enabled) return;
-    // same test as subtile_cull(), with everything that does not depend on the tile hoisted out of the loop
+    // lgr::rect_culled per tile, with everything that does not depend on the tile hoisted out of the loop
     const float A = co.x, B = co.y, Cc = co.z;
     const float t = 257.55f * co.w;
     if (t <= 1.0f) {  // alpha <= opacity < 1/255 everywhere: the Gaussian is listed nowhere
@@ -379,23 +367,9 @@ __device__ __forceinline__ void tile_keep_mask(const lgr::Geom& geo, float4 co, 
     int b = 0;
     for (int ty = geo.rect.y0; ty < geo.rect.y1; ty++) {
         const float dy_lo = geo.py - (float)min(ty * LGR_TILE + LGR_TILE - 1, H - 1), dy_hi = geo.py - (float)(ty * LGR_TILE);
-        const float cy = fminf(fmaxf(0.f, dy_lo), dy_hi);
         for (int tx = geo.rect.x0; tx < geo.rect.x1; tx++, b++) {
             const float dx_lo = geo.px - (float)min(tx * LGR_TILE + LGR_TILE - 1, W - 1), dx_hi = geo.px - (float)(tx * LGR_TILE);
-            const float cx = fminf(fmaxf(0.f, dx_lo), dx_hi);
-            float q = 0.f;
-            if (cx != 0.f || cy != 0.f) {
-                q = 3.0e38f;
-                if (cx != 0.f) {
-                    const float dy = fminf(fmaxf(nbc * cx, dy_lo), dy_hi);
-                    q = hA * cx * cx + hC * dy * dy + B * cx * dy;
-                }
-                if (cy != 0.f) {
-                    const float dx = fminf(fmaxf(nba * cy, dx_lo), dx_hi);
-                    q = fminf(q, hA * dx * dx + hC * cy * cy + B * dx * cy);
-                }
-            }
-            if (!(q > thr)) m |= 1ull << b;
+            if (!lgr::rect_culled(hA, hC, B, nba, nbc, thr, dx_lo, dx_hi, dy_lo, dy_hi)) m |= 1ull << b;
         }
     }
     mask = m;
@@ -429,7 +403,8 @@ __device__ __forceinline__ unsigned long long warp_tile_keep_mask(bool visible, 
     if (total == 0) return mask;
     const float thr = __logf(fmaxf(t, 1.0f));
     const float nbc = __fdividef(-B, Cc), nba = __fdividef(-B, A), hA = 0.5f * A, hC = 0.5f * Cc;
-    const int packed = visible ? (geo.rect.x0 | (geo.rect.y0 << 12) | (w << 24)) : (1 << 24);   // w <= 64 here; x0, y0 < 4096 tiles
+    // the rectangle's origin and width travel unpacked, so any tile index works; idle lanes get width 1 (never a division by 0)
+    const int x0 = visible ? geo.rect.x0 : 0, y0 = visible ? geo.rect.y0 : 0, width = visible ? w : 1;
     const float px = visible ? geo.px : 0.f, py = visible ? geo.py : 0.f;
     unsigned long long kept = 0ull;
     for (uint32_t base = 0; base < total; base += 32) {
@@ -443,32 +418,18 @@ __device__ __forceinline__ unsigned long long warp_tile_keep_mask(bool visible, 
             else hi = mid - 1;
         }
         const uint32_t o_off = __shfl_sync(FULL, off, lo);
-        const int o_pk = __shfl_sync(FULL, packed, lo);
+        const int o_x0 = __shfl_sync(FULL, x0, lo), o_y0 = __shfl_sync(FULL, y0, lo), o_w = __shfl_sync(FULL, width, lo);
         const float o_px = __shfl_sync(FULL, px, lo), o_py = __shfl_sync(FULL, py, lo);
         const float o_hA = __shfl_sync(FULL, hA, lo), o_hC = __shfl_sync(FULL, hC, lo), o_B = __shfl_sync(FULL, B, lo);
         const float o_nbc = __shfl_sync(FULL, nbc, lo), o_nba = __shfl_sync(FULL, nba, lo), o_thr = __shfl_sync(FULL, thr, lo);
         bool keep = false;
         if (j < total) {
-            const int o_w = (o_pk >> 24) & 0xff, local = (int)(j - o_off);
+            const int local = (int)(j - o_off);
             const int ry = (int)__fdividef((float)local + 0.5f, (float)o_w), rx = local - ry * o_w;
-            const int tx = (o_pk & 0xfff) + rx, ty = ((o_pk >> 12) & 0xfff) + ry;
+            const int tx = o_x0 + rx, ty = o_y0 + ry;
             const float dy_lo = o_py - (float)min(ty * LGR_TILE + LGR_TILE - 1, H - 1), dy_hi = o_py - (float)(ty * LGR_TILE);
-            const float cy = fminf(fmaxf(0.f, dy_lo), dy_hi);
             const float dx_lo = o_px - (float)min(tx * LGR_TILE + LGR_TILE - 1, W - 1), dx_hi = o_px - (float)(tx * LGR_TILE);
-            const float cx = fminf(fmaxf(0.f, dx_lo), dx_hi);
-            float q = 0.f;
-            if (cx != 0.f || cy != 0.f) {
-                q = 3.0e38f;
-                if (cx != 0.f) {
-                    const float dy = fminf(fmaxf(o_nbc * cx, dy_lo), dy_hi);
-                    q = o_hA * cx * cx + o_hC * dy * dy + o_B * cx * dy;
-                }
-                if (cy != 0.f) {
-                    const float dx = fminf(fmaxf(o_nba * cy, dx_lo), dx_hi);
-                    q = fminf(q, o_hA * dx * dx + o_hC * cy * cy + o_B * dx * cy);
-                }
-            }
-            keep = !(q > o_thr);
+            keep = !lgr::rect_culled(o_hA, o_hC, o_B, o_nba, o_nbc, o_thr, dx_lo, dx_hi, dy_lo, dy_hi);
         }
         const unsigned bal = __ballot_sync(FULL, keep);
         // my candidates inside [base, base + 32)

@@ -48,6 +48,36 @@ void mh_preprocess(int P, int D, int M, const float* means3D, const float* scale
 
 float mh_pair_power(float dx, float dy, float A, float B, float C) { return lgr::pair_power(dx, dy, A, B, C); }
 
+// For each of n (Gaussian, pixel rectangle) pairs: the largest pinned pair_power over the pixel centres x0..x1, y0..y1 (inclusive) at
+// which the reference blends at all (power <= 0), -inf when there is none.  The reference blends a pixel when o * exp(power) >= 1/255.
+void mh_rect_max_power(int n, const float* px, const float* py, const float* A, const float* B, const float* C, const int32_t* x0,
+                       const int32_t* x1, const int32_t* y0, const int32_t* y1, float* out)
+{
+    for (int i = 0; i < n; i++) {
+        float best = -INFINITY;
+        for (int y = y0[i]; y <= y1[i]; y++)
+            for (int x = x0[i]; x <= x1[i]; x++) {
+                const float p = lgr::pair_power(px[i] - (float)x, py[i] - (float)y, A[i], B[i], C[i]);
+                if (p <= 0.0f && p > best) best = p;
+            }
+        out[i] = best;
+    }
+}
+
+// The binning-time tile cull on the host, with the per-Gaussian set-up of tile_keep_mask (lgrast.cu): culled[i] = rect_culled over the
+// pixel centres x0..x1, y0..y1, and the rect_qmin q and mag it compared.
+void mh_rect_cull(int n, const float* px, const float* py, const float* A, const float* B, const float* C, const float* o, const int32_t* x0,
+                  const int32_t* x1, const int32_t* y0, const int32_t* y1, uint8_t* culled, float* q, float* mag)
+{
+    for (int i = 0; i < n; i++) {
+        const float thr = logf(257.55f * o[i]);
+        const float hA = 0.5f * A[i], hC = 0.5f * C[i], nba = -B[i] / A[i], nbc = -B[i] / C[i];
+        const float dx_lo = px[i] - (float)x1[i], dx_hi = px[i] - (float)x0[i], dy_lo = py[i] - (float)y1[i], dy_hi = py[i] - (float)y0[i];
+        lgr::rect_qmin(hA, hC, B[i], nba, nbc, dx_lo, dx_hi, dy_lo, dy_hi, q[i], mag[i]);
+        culled[i] = lgr::rect_culled(hA, hC, B[i], nba, nbc, thr, dx_lo, dx_hi, dy_lo, dy_hi) ? 1 : 0;
+    }
+}
+
 // K7+K8 on the host: the same helper sequence preprocess_backward_kernel runs per Gaussian.
 void mh_preprocess_backward(int P, int D, int M, const float* means3D, const int32_t* radii, const float* shs, const uint8_t* clamped,
                             const float* scales, const float* rotations, float mod, const float* cov3D, const float* view,
