@@ -9,9 +9,12 @@ try:  # render.py:22 / render_video.py:23 do `from gaussian_renderer import Gaus
 except Exception:  # reference checkout not on the path: the name is simply absent
     GaussianModel = None
 
+if _os.environ.get("LGR_SELECTIVE_ADAM", "0") == "1" and _os.environ.get("LGR_FUSED_OPTIM", "1") == "0":
+    raise RuntimeError("LGR_SELECTIVE_ADAM=1 needs the fused optimizer: it cannot be combined with LGR_FUSED_OPTIM=0")
 if GaussianModel is not None and _os.environ.get("LGR_FUSED_OPTIM", "1") != "0":
     # row N3: the AdamW built by GaussianModel.training_setup becomes FusedAdamW (bit-identical updates, one launch per step)
     # and prune_points uses the fused compaction; LGR_FUSED_OPTIM=0 keeps torch.optim.AdamW and the reference's surgery.
+    # LGR_SELECTIVE_ADAM=1 makes it a SelectiveAdamW (opt-in: only Gaussians with a non-zero gradient row are stepped).
     from lightgaussian_b200 import optim as _optim
     _optim.install(GaussianModel)
 if GaussianModel is not None and hasattr(GaussianModel, "load_vq") and _os.environ.get("LGR_FUSED", "1") != "0":

@@ -276,6 +276,28 @@ typedef struct lgr_adamw_tensor {
 int lgr_adamw_step(int n_tensors, const lgr_adamw_tensor* tensors, double beta1, double beta2, double eps, double weight_decay,
                    void* cuda_stream);
 
+/* lgr_adamw_step_selective: the same update, restricted to the ACTIVE rows.  All tensors share `rows` in dim 0 (one row per
+ * Gaussian); row i is active when any element of row i of any tensor's gradient compares unequal to zero (+0 and -0 do not, NaN
+ * does).  Every element of an active row is updated bit-identically to lgr_adamw_step; the parameter and both moments of an inactive
+ * row are neither read nor written.  Each array is a [rows, width] view: element (r, c) lives at base[r * row_stride + c * col_stride]
+ * (dense [P, ...]: (width, 1); a row-strided view: (its row stride, 1); the permuted dense _xyz of create_from_pcd: (1, P)).  At most
+ * 8 tensors whose widths add up to at most 400 floats per row; width 0 = the tensor takes no part; rows == 0 launches nothing. */
+typedef struct lgr_adamw_row_tensor {
+    float* param;
+    const float* grad;
+    float* exp_avg;
+    float* exp_avg_sq;
+    int64_t width;                  /* elements per row */
+    int64_t param_row_stride, param_col_stride;
+    int64_t grad_row_stride, grad_col_stride;
+    int64_t exp_avg_row_stride, exp_avg_col_stride;
+    int64_t exp_avg_sq_row_stride, exp_avg_sq_col_stride;
+    double lr;
+    double step;                    /* step count AFTER the increment, as lgr_adamw_tensor.step */
+} lgr_adamw_row_tensor;
+int lgr_adamw_step_selective(int n_tensors, const lgr_adamw_row_tensor* tensors, long long rows, double beta1, double beta2, double eps,
+                             double weight_decay, void* cuda_stream);
+
 /* Row compaction of GaussianModel._prune_optimizer / prune_points (scene/gaussian_model.py:564-600): `keep` is a device byte
  * mask over P rows.  lgr_compact_plan writes the indices of the kept rows, ascending, to src_row[0..rows_out) and returns
  * rows_out through a host pointer (one stream synchronisation); lgr_compact_rows then gathers up to 24 row-major tensors

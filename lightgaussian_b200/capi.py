@@ -54,6 +54,14 @@ class LgrAdamwTensor(C.Structure):
                 ("numel", C.c_int64), ("lr", C.c_double), ("step", C.c_double), ("row_elems", C.c_int64), ("param_row_stride", C.c_int64)]
 
 
+class LgrAdamwRowTensor(C.Structure):
+    """struct lgr_adamw_row_tensor"""
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("width", C.c_int64),
+                ("param_row_stride", C.c_int64), ("param_col_stride", C.c_int64), ("grad_row_stride", C.c_int64), ("grad_col_stride", C.c_int64),
+                ("exp_avg_row_stride", C.c_int64), ("exp_avg_col_stride", C.c_int64),
+                ("exp_avg_sq_row_stride", C.c_int64), ("exp_avg_sq_col_stride", C.c_int64), ("lr", C.c_double), ("step", C.c_double)]
+
+
 class LgrCompactTensor(C.Structure):
     """struct lgr_compact_tensor"""
     _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("row_words", C.c_int32)]
@@ -136,6 +144,9 @@ def load():
         lib.lgr_image_loss_backward.argtypes = [vp, vp, vp, i32, i32, i32, C.c_float, C.c_float, vp, vp, vp]
         lib.lgr_adamw_step.restype = i32
         lib.lgr_adamw_step.argtypes = [i32, C.POINTER(LgrAdamwTensor), C.c_double, C.c_double, C.c_double, C.c_double, vp]
+        lib.lgr_adamw_step_selective.restype = i32
+        lib.lgr_adamw_step_selective.argtypes = [i32, C.POINTER(LgrAdamwRowTensor), C.c_longlong, C.c_double, C.c_double, C.c_double,
+                                                 C.c_double, vp]
         lib.lgr_compact_workspace_bytes.restype = C.c_size_t
         lib.lgr_compact_workspace_bytes.argtypes = [i32]
         lib.lgr_compact_plan.restype = i32

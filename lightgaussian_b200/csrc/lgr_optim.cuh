@@ -3,6 +3,7 @@
 //                          (scene/gaussian_model.py:184-217) as ONE launch: every tensor of every group is a row of a
 //                          pointer table, a block handles one 4096-element chunk of one tensor.  28 B of HBM traffic per
 //                          element (read p,g,m,v; write p,m,v) against ~80 B for the ~9 foreach passes torch launches per group.
+//   * adamw_selective_kernel  the same update on the rows (Gaussians) whose gradient is not all zero only (opt-in SelectiveAdamW).
 //   * compact_gather_kernel  the row compaction of GaussianModel._prune_optimizer / prune_points (:564-600): parameters and both
 //                          Adam moments of all groups gathered through one source-row index in one launch (the reference does
 //                          18 boolean-mask indexings, each with its own nonzero() and host synchronisation).
@@ -145,6 +146,140 @@ __global__ void __launch_bounds__(256) adamw_multi_kernel(const AdamTable t)
             float p = P[e], m = M[e], v = V[e];
             adamw_element(p, G[e], m, v, decay, neg_step, bc2, t.w1, t.beta2, t.w2, t.eps);
             P[e] = p; M[e] = m; V[e] = v;
+        }
+    }
+}
+
+// ---- selective AdamW: only the rows (Gaussians) with a non-zero gradient -------------------------------------------------
+// Every tensor is a [rows, width] view with its own (row stride, column stride) per array: dense [P, ...] is (width, 1), the
+// distillation student's _features_rest[:, :8, :] is (45, 1) for the parameter and (24, 1) for its dense gradient and moments, the
+// permuted _xyz of create_from_pcd is (1, P).  A block owns SEL_ROWS rows:
+//   1. the gradient slice of every tensor for those rows goes to shared memory ([SEL_ROWS][width] per tensor) -- one TMA bulk copy
+//      per tensor when the slice is one 16-byte aligned span (row-contiguous gradients), plain streaming loads otherwise;
+//   2. a row is active when any element of it, in any tensor, compares unequal to zero (+0 and -0 do not, NaN does); one ballot per
+//      warp and a 4-entry prefix turn the flags into an ascending list of active rows;
+//   3. only the active rows are walked: p, m, v loaded, adamw_element (the dense kernel's arithmetic, unchanged), stored back.
+// Inactive rows are never read or written.  Traffic: the gradients once, plus 24 B per element of the active rows.
+constexpr int SEL_ROWS = 128;
+constexpr int SEL_THREADS = 256;
+constexpr int SEL_MAX_ROW_FLOATS = 400;       // sum of the widths: SEL_ROWS * 400 * 4 B = 200 KB of shared memory at most
+
+struct SelAdamTable {
+    float* p[OPT_MAX_TENSORS];
+    const float* g[OPT_MAX_TENSORS];
+    float* m[OPT_MAX_TENSORS];
+    float* v[OPT_MAX_TENSORS];
+    long long rs[OPT_MAX_TENSORS][4];       // row strides of p, g, m, v (elements)
+    long long cs[OPT_MAX_TENSORS][4];       // column strides of p, g, m, v (elements)
+    int width[OPT_MAX_TENSORS];
+    int smem_off[OPT_MAX_TENSORS];          // float offset of the tensor's [SEL_ROWS][width] gradient slice in shared memory
+    float decay[OPT_MAX_TENSORS];           // as AdamTable
+    float neg_step[OPT_MAX_TENSORS];
+    float bc2_sqrt[OPT_MAX_TENSORS];
+    float w1, beta2, w2, eps;
+    long long rows;
+    int count;
+};
+
+__global__ void __launch_bounds__(SEL_THREADS) adamw_selective_kernel(const SelAdamTable t)
+{
+    extern __shared__ __align__(16) float sel_grad[];
+    __shared__ __align__(8) uint64_t bar;
+    __shared__ int active_list[SEL_ROWS];
+    __shared__ int warp_active[SEL_ROWS / 32];
+
+    const long long r0 = (long long)blockIdx.x * SEL_ROWS;
+    const int nr = (int)min((long long)SEL_ROWS, t.rows - r0);
+    const int tid = threadIdx.x;
+
+    // 1. gradient slices -> shared memory
+    uint32_t bulk_bytes = 0;
+    for (int k = 0; k < t.count; k++) {
+        const int w = t.width[k];
+        const float* src = t.g[k] + r0 * t.rs[k][1];
+        const uint32_t bytes = (uint32_t)(nr * w) * 4u;
+        if (t.cs[k][1] == 1 && t.rs[k][1] == w && ((reinterpret_cast<uintptr_t>(src) | bytes) & 15) == 0) {
+            bulk_bytes += bytes;
+            continue;
+        }
+        float* dst = sel_grad + t.smem_off[k];
+        const long long rs = t.rs[k][1], cs = t.cs[k][1];
+        if (cs == 1) {
+            for (int e = tid; e < nr * w; e += SEL_THREADS) {
+                const int r = e / w, c = e - r * w;
+                dst[e] = __ldcs(src + r * rs + c);
+            }
+        } else {   // column-major walk: consecutive threads read consecutive rows of one column (the permuted _xyz)
+            for (int e = tid; e < nr * w; e += SEL_THREADS) {
+                const int c = e / nr, r = e - c * nr;
+                dst[r * w + c] = __ldcs(src + r * rs + c * cs);
+            }
+        }
+    }
+    if (tid == 0 && bulk_bytes) {
+        mbar_init(&bar, 1);
+        fence_mbar_init();
+        mbar_expect_tx(&bar, bulk_bytes);
+        for (int k = 0; k < t.count; k++) {
+            const int w = t.width[k];
+            const float* src = t.g[k] + r0 * t.rs[k][1];
+            const uint32_t bytes = (uint32_t)(nr * w) * 4u;
+            if (t.cs[k][1] == 1 && t.rs[k][1] == w && ((reinterpret_cast<uintptr_t>(src) | bytes) & 15) == 0)
+                bulk_g2s(sel_grad + t.smem_off[k], src, bytes, &bar);
+        }
+    }
+    __syncthreads();                 // plain loads visible; the barrier is initialised before anyone waits on it
+    if (bulk_bytes) mbar_wait(&bar, 0);
+
+    // 2. active rows -> ascending list
+    bool active = false;
+    if (tid < nr) {
+        for (int k = 0; k < t.count; k++) {
+            const int w = t.width[k];
+            const float* row = sel_grad + t.smem_off[k] + tid * w;
+            for (int c = 0; c < w; c++) active |= row[c] != 0.f;
+        }
+    }
+    const int lane = tid & 31, warp = tid >> 5;
+    int rank = 0;
+    if (warp < SEL_ROWS / 32) {
+        const unsigned bal = __ballot_sync(FULL, active);
+        rank = __popc(bal & ((1u << lane) - 1u));
+        if (lane == 0) warp_active[warp] = __popc(bal);
+    }
+    __syncthreads();
+    int n_active = 0, base = 0;
+#pragma unroll
+    for (int i = 0; i < SEL_ROWS / 32; i++) {
+        if (i < warp) base += warp_active[i];
+        n_active += warp_active[i];
+    }
+    if (active) active_list[base + rank] = tid;
+    __syncthreads();
+    if (n_active == 0) return;
+
+    // 3. AdamW on the active rows only
+    for (int k = 0; k < t.count; k++) {
+        const int w = t.width[k];
+        const float* G = sel_grad + t.smem_off[k];
+        float* __restrict__ P = t.p[k];
+        float* __restrict__ M = t.m[k];
+        float* __restrict__ V = t.v[k];
+        const long long rsp = t.rs[k][0], csp = t.cs[k][0], rsm = t.rs[k][2], csm = t.cs[k][2], rsv = t.rs[k][3], csv = t.cs[k][3];
+        const float decay = t.decay[k], neg_step = t.neg_step[k], bc2 = t.bc2_sqrt[k];
+        const bool by_column = csp != 1;   // permuted layouts: walk column by column so that a warp reads consecutive rows
+        for (int e = tid; e < n_active * w; e += SEL_THREADS) {
+            int i, c;
+            if (by_column) { c = e / n_active; i = e - c * n_active; }
+            else           { i = e / w; c = e - i * w; }
+            const int r = active_list[i];
+            const long long row = r0 + r;
+            float* pp = P + row * rsp + c * csp;
+            float* mp = M + row * rsm + c * csm;
+            float* vp = V + row * rsv + c * csv;
+            float p = *pp, m = *mp, v = *vp;
+            adamw_element(p, G[r * w + c], m, v, decay, neg_step, bc2, t.w1, t.beta2, t.w2, t.eps);
+            *pp = p; *mp = m; *vp = v;
         }
     }
 }

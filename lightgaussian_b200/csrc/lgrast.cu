@@ -63,14 +63,14 @@ std::atomic<uint64_t> g_launches{0};
 
 // ---- optional per-stage device timing (CUDA events on the launch stream), used by bench.py's roofline ----
 enum StageId { ST_PREPROCESS = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_TILE_SORT, ST_RANGES, ST_BLEND_FWD, ST_BLEND_FWD_COUNT,
-               ST_SCORE, ST_BLEND_BWD, ST_PREPROCESS_BWD, ST_MEMSET, ST_SH_GRAD, ST_PEER_ALLREDUCE, ST_LOSS_FWD, ST_LOSS_BWD, ST_ADAMW, ST_COMPACT, ST_VQ_ASSIGN, ST_VQ_UPDATE, ST_SPARSE_PACK, ST_SPARSE_ACC, ST_BIN_DSORT, ST_BIN_COUNT, ST_BIN_SCATTER, ST_DET_GATHER, ST_COUNT };
+               ST_SCORE, ST_BLEND_BWD, ST_PREPROCESS_BWD, ST_MEMSET, ST_SH_GRAD, ST_PEER_ALLREDUCE, ST_LOSS_FWD, ST_LOSS_BWD, ST_ADAMW, ST_COMPACT, ST_VQ_ASSIGN, ST_VQ_UPDATE, ST_SPARSE_PACK, ST_SPARSE_ACC, ST_BIN_DSORT, ST_BIN_COUNT, ST_BIN_SCATTER, ST_DET_GATHER, ST_ADAMW_SELECTIVE, ST_COUNT };
 const char* const kStageNames[ST_COUNT] = {"preprocess_kernel", "depth_sort(cub)", "scan(cub)", "emit_kernel", "tile_sort(cub)",
                                            "ranges_kernel", "blend_forward_kernel", "blend_forward_kernel<count>", "score_kernel",
                                            "blend_backward_kernel", "preprocess_backward_kernel", "memset", "sh_grad_from_views_kernel",
                                            "peer_allreduce_kernel", "image_loss_forward_kernel", "image_loss_backward_kernel", "adamw_multi_kernel",
                                            "compact_gather_kernel", "vq_assign_kernel", "vq_ema_kernels", "sparse_pack(flag+scan+index+K8)",
                                            "sparse_accumulate_kernel", "depth_sort(dsort_count+bin_scan+dsort_scatter x3)", "tile_count_kernel+bin_scan_kernel",
-                                           "tile_scatter_kernel", "det_gather_kernel"};
+                                           "tile_scatter_kernel", "det_gather_kernel", "adamw_selective_kernel"};
 struct ProfRecord { int stage; cudaEvent_t a, b; };
 bool g_prof_on = false;
 std::vector<ProfRecord> g_prof_records;
@@ -2240,6 +2240,16 @@ int lgr_image_loss_backward(const float* img, const float* target, const float* 
 }
 
 // ---- optimizer (row N3) ----
+// the per-tensor host scalars of one AdamW step: torch/optim/adam.py _multi_tensor_adam forms them from python floats (double), then
+// casts them to the kernels' opmath type (float)
+static void adamw_scalars(double lr, double step, double beta1, double beta2, double weight_decay, float* decay, float* neg_step, float* bc2_sqrt)
+{
+    const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
+    *decay = (float)(1.0 - lr * weight_decay);
+    *neg_step = (float)((lr / bc1) * -1.0);
+    *bc2_sqrt = (float)pow(bc2, 0.5);
+}
+
 int lgr_adamw_step(int n_tensors, const lgr_adamw_tensor* tensors, double beta1, double beta2, double eps, double weight_decay,
                    void* cuda_stream)
 {
@@ -2258,8 +2268,6 @@ int lgr_adamw_step(int n_tensors, const lgr_adamw_tensor* tensors, double beta1,
             g_last_error = "lgr_adamw_step: tensor with a missing pointer, negative size or step < 1";
             return LGR_ERR_INVALID_ARG;
         }
-        // torch/optim/adam.py _multi_tensor_adam: python floats (double), then cast to the kernels' opmath type (float)
-        const double bc1 = 1.0 - pow(beta1, a.step), bc2 = 1.0 - pow(beta2, a.step);
         t.p[k] = a.param; t.g[k] = a.grad; t.m[k] = a.exp_avg; t.v[k] = a.exp_avg_sq;
         t.n[k] = a.numel;
         if (a.row_elems < 0 || a.row_elems > 0x7fffffffLL || (a.row_elems > 0 && (a.param_row_stride < a.row_elems || a.param_row_stride > 0x7fffffffLL ||
@@ -2269,9 +2277,7 @@ int lgr_adamw_step(int n_tensors, const lgr_adamw_tensor* tensors, double beta1,
         }
         t.row_elems[k] = (a.row_elems > 0 && a.param_row_stride != a.row_elems) ? (int)a.row_elems : 0;
         t.row_stride[k] = (int)a.param_row_stride;
-        t.decay[k] = (float)(1.0 - a.lr * weight_decay);
-        t.neg_step[k] = (float)((a.lr / bc1) * -1.0);
-        t.bc2_sqrt[k] = (float)pow(bc2, 0.5);
+        adamw_scalars(a.lr, a.step, beta1, beta2, weight_decay, &t.decay[k], &t.neg_step[k], &t.bc2_sqrt[k]);
         t.chunk_start[k] = (int)chunks;
         chunks += (a.numel + OPT_CHUNK - 1) / OPT_CHUNK;
         k++;
@@ -2290,6 +2296,75 @@ int lgr_adamw_step(int n_tensors, const lgr_adamw_tensor* tensors, double beta1,
         adamw_multi_kernel<<<(unsigned)chunks, 256, 0, stream>>>(t);
     }
     LGR_LAUNCH_CHECK("adamw_multi_kernel", false, stream);
+    return LGR_OK;
+}
+
+// the [rows, width] view (row stride rs, column stride cs) reaches no element twice: rows lie side by side (cs*width <= rs) or
+// columns do (rs*rows <= cs)
+static bool row_view_ok(long long rows, long long width, long long rs, long long cs)
+{
+    if (rs < 0 || cs < 0 || rs > (1LL << 40) || cs > (1LL << 40)) return false;
+    if (rows > 1 && width > 1) return (cs >= 1 && cs * width <= rs) || (rs >= 1 && rs * rows <= cs);
+    if (rows > 1) return rs >= 1;
+    if (width > 1) return cs >= 1;
+    return true;
+}
+
+int lgr_adamw_step_selective(int n_tensors, const lgr_adamw_row_tensor* tensors, long long rows, double beta1, double beta2, double eps,
+                             double weight_decay, void* cuda_stream)
+{
+    if (n_tensors < 0 || n_tensors > OPT_MAX_TENSORS || (n_tensors && !tensors) || rows < 0 || rows > (1LL << 37)) {
+        g_last_error = "lgr_adamw_step_selective: between 0 and 8 tensors per call and 0 <= rows < 2^37";
+        return LGR_ERR_INVALID_ARG;
+    }
+    SelAdamTable t;
+    memset(&t, 0, sizeof(t));
+    int k = 0, row_floats = 0;
+    for (int i = 0; i < n_tensors; i++) {
+        const lgr_adamw_row_tensor& a = tensors[i];
+        if (a.width < 0 || a.width > SEL_MAX_ROW_FLOATS) {
+            g_last_error = "lgr_adamw_step_selective: width must be between 0 and 400";
+            return LGR_ERR_INVALID_ARG;
+        }
+        if (a.width == 0 || rows == 0) continue;
+        if (!a.param || !a.grad || !a.exp_avg || !a.exp_avg_sq || a.step < 1.0) {
+            g_last_error = "lgr_adamw_step_selective: tensor with a missing pointer or step < 1";
+            return LGR_ERR_INVALID_ARG;
+        }
+        const long long rs[4] = {a.param_row_stride, a.grad_row_stride, a.exp_avg_row_stride, a.exp_avg_sq_row_stride};
+        const long long cs[4] = {a.param_col_stride, a.grad_col_stride, a.exp_avg_col_stride, a.exp_avg_sq_col_stride};
+        for (int j = 0; j < 4; j++) {
+            if (!row_view_ok(rows, a.width, rs[j], cs[j])) {
+                g_last_error = "lgr_adamw_step_selective: a [rows, width] view whose strides overlap its own elements or are negative";
+                return LGR_ERR_INVALID_ARG;
+            }
+            t.rs[k][j] = rs[j];
+            t.cs[k][j] = cs[j];
+        }
+        row_floats += (int)a.width;
+        if (row_floats > SEL_MAX_ROW_FLOATS) {
+            g_last_error = "lgr_adamw_step_selective: the widths add up to more than 400 floats per row";
+            return LGR_ERR_INVALID_ARG;
+        }
+        t.p[k] = a.param; t.g[k] = a.grad; t.m[k] = a.exp_avg; t.v[k] = a.exp_avg_sq;
+        t.width[k] = (int)a.width;
+        t.smem_off[k] = (row_floats - (int)a.width) * SEL_ROWS;
+        adamw_scalars(a.lr, a.step, beta1, beta2, weight_decay, &t.decay[k], &t.neg_step[k], &t.bc2_sqrt[k]);
+        k++;
+    }
+    t.count = k;
+    t.rows = rows;
+    t.w1 = (float)(1.0 - beta1); t.beta2 = (float)beta2; t.w2 = (float)(1.0 - beta2); t.eps = (float)eps;
+    if (k == 0) return LGR_OK;
+    const size_t smem = (size_t)row_floats * SEL_ROWS * sizeof(float);
+    // always: static + dynamic shared memory together may pass 48 KB even when the dynamic part alone does not
+    LGR_CUDA_TRY(cudaFuncSetAttribute(adamw_selective_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(smem, (size_t)48 * 1024)));
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    {
+        ProfScope ps(ST_ADAMW_SELECTIVE, stream);
+        adamw_selective_kernel<<<(unsigned)((rows + SEL_ROWS - 1) / SEL_ROWS), SEL_THREADS, smem, stream>>>(t);
+    }
+    LGR_LAUNCH_CHECK("adamw_selective_kernel", false, stream);
     return LGR_OK;
 }
 

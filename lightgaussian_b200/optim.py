@@ -7,12 +7,16 @@ builds its optimizer as `torch.optim.AdamW(l, lr=0.0, eps=1e-15)` over six group
 (scene/gaussian_model.py:184-217) and only ever touches `state[p]["exp_avg"]`, `state[p]["exp_avg_sq"]`, `param_groups[i]["lr"]`,
 `["params"][0]`, `["name"]` and `state_dict()` afterwards (:219-225, :544-660) -- all of which this class keeps.
 
+`SelectiveAdamW` (opt-in, `LGR_SELECTIVE_ADAM=1`) is the same optimizer restricted to the Gaussians whose gradient row is not all
+zero (`lgr_adamw_step_selective`); the rows a step did not reach keep their parameters and moments untouched.
+
 `compact_rows` / `prune_points` are the fused form of `GaussianModel._prune_optimizer` + `prune_points` (:564-600): one stream
 compaction of the mask, then ONE gather launch for the parameters and both Adam moments of every group.
 """
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import torch
 
@@ -37,6 +41,23 @@ class FusedAdamW(torch.optim.AdamW):
                 loss = closure()
         lib = capi.load()
         trace.bump("adamw_steps")
+        for (device, beta1, beta2, eps, wd), items in self._prepare().items():
+            for i0 in range(0, len(items), 8):
+                chunk = items[i0:i0 + 8]
+                arr = (capi.LgrAdamwTensor * len(chunk))()
+                for a, (p, g, m, v, lr, step, row_elems, row_stride) in zip(arr, chunk):
+                    a.param, a.grad, a.exp_avg, a.exp_avg_sq = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
+                    a.numel, a.lr, a.step = p.numel(), lr, step
+                    a.row_elems, a.param_row_stride = row_elems, row_stride
+                with torch.cuda.device(device):
+                    st = lib.lgr_adamw_step(len(chunk), arr, beta1, beta2, eps, wd, capi.current_stream_ptr(device))
+                capi.check(st, "lgr_adamw_step")
+        return loss
+
+    def _prepare(self):
+        """Checks every parameter with a gradient, creates its state on first use and increments its step, as torch's AdamW does.
+        Returns {(device, beta1, beta2, eps, weight_decay): [(p, g, m, v, lr, step, row_elems, row_stride)]} with every gradient in a
+        layout the kernels take."""
         by_cfg = {}
         for group in self.param_groups:
             if isinstance(group["lr"], torch.Tensor):
@@ -79,19 +100,70 @@ class FusedAdamW(torch.optim.AdamW):
                         raise RuntimeError("FusedAdamW: optimizer state must be contiguous")
                 key = (p.device, float(beta1), float(beta2), float(group["eps"]), float(group["weight_decay"]))
                 by_cfg.setdefault(key, []).append((p, g, m, v, float(group["lr"]), float(state["step"]), row_elems, row_stride))
-        for (device, beta1, beta2, eps, wd), items in by_cfg.items():
-            for i0 in range(0, len(items), 8):
-                chunk = items[i0:i0 + 8]
-                arr = (capi.LgrAdamwTensor * len(chunk))()
-                for a, (p, g, m, v, lr, step, row_elems, row_stride) in zip(arr, chunk):
-                    a.param, a.grad, a.exp_avg, a.exp_avg_sq = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
-                    a.numel, a.lr, a.step = p.numel(), lr, step
-                    a.row_elems, a.param_row_stride = row_elems, row_stride
-                with torch.cuda.device(device):
-                    st = lib.lgr_adamw_step(len(chunk), arr, beta1, beta2, eps, wd, capi.current_stream_ptr(device))
-                capi.check(st, "lgr_adamw_step")
+        return by_cfg
+
+
+class SelectiveAdamW(FusedAdamW):
+    """FusedAdamW that updates only the Gaussians a step reached: the selective (sparse) Adam of Taming-3DGS and gsplat's
+    SelectiveAdam, with the mask taken from the gradients themselves.  Opt-in: results differ from torch's AdamW by design.
+
+    Every parameter with a gradient must have the same number of rows P (one per Gaussian).  Row i is active when any element of
+    row i of any of those gradients is not equal to zero (+0 and -0 are zero; a NaN makes the row active).  Every element of an active
+    row is updated bit-identically to FusedAdamW / torch.optim.AdamW with its group's hyper-parameters and step count; the parameter,
+    exp_avg and exp_avg_sq of an inactive row are left untouched (no momentum step, no weight decay).  state["step"] is incremented
+    for every parameter with a gradient, whichever rows were active, so a row that wakes up uses the global step for bias correction.
+    Same constructor, state layout and state_dict as torch.optim.AdamW: checkpoints move freely between the three.  The groups must
+    share betas, eps and weight_decay (the reference's six groups differ only in lr)."""
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        # everything that can refuse the step does so before any state changes
+        live = [(g, p) for g in self.param_groups for p in g["params"] if p.grad is not None]
+        rows = {p.shape[0] if p.dim() else 1 for _, p in live}
+        if len(rows) > 1:
+            raise RuntimeError(f"SelectiveAdamW: parameters with a gradient must share their number of rows, got {sorted(rows)}")
+        if len({(float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"])) for g, _ in live}) > 1:
+            raise NotImplementedError("SelectiveAdamW: all groups must share betas, eps and weight_decay")
+        if len({p.device for _, p in live}) > 1 or len(live) > 8:
+            raise NotImplementedError("SelectiveAdamW: at most 8 parameters with a gradient, on one device (one row mask spans them all)")
+        for _, p in live:
+            if p.numel():
+                _row_view(p)     # _prepare gives the gradient and the moments this layout or a contiguous one
+        lib = capi.load()
+        trace.bump("adamw_selective_steps")
+        for (device, beta1, beta2, eps, wd), items in self._prepare().items():
+            P = rows.pop()
+            arr = (capi.LgrAdamwRowTensor * len(items))()
+            for a, (p, g, m, v, lr, step, _, _) in zip(arr, items):
+                a.param, a.grad, a.exp_avg, a.exp_avg_sq = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
+                a.width, a.lr, a.step = (p.numel() // P) if P else 0, lr, step
+                if a.width:
+                    a.param_row_stride, a.param_col_stride = _row_view(p)
+                    a.grad_row_stride, a.grad_col_stride = _row_view(g, p)
+                    a.exp_avg_row_stride, a.exp_avg_col_stride = _row_view(m, p)
+                    a.exp_avg_sq_row_stride, a.exp_avg_sq_col_stride = _row_view(v, p)
+            with torch.cuda.device(device):
+                st = lib.lgr_adamw_step_selective(len(items), arr, P, beta1, beta2, eps, wd, capi.current_stream_ptr(device))
+            capi.check(st, "lgr_adamw_step_selective")
         return loss
 
+
+def _row_view(t, like=None):
+    """(row stride, column stride) of `t` seen as [P, width]: column c is the c-th element of a row in the memory order of the
+    parameter `like` (default: `t` itself), so that p, g, m and v pair up element by element.  Raises when the non-row dimensions
+    do not flatten to one column stride."""
+    order = sorted((d for d in range(1, t.dim()) if t.size(d) != 1), key=(like if like is not None else t).stride)
+    cs = t.stride(order[0]) if order else 1
+    expect = cs
+    for d in order:
+        if t.stride(d) != expect:
+            raise RuntimeError(f"SelectiveAdamW: a tensor of shape {tuple(t.shape)} and strides {t.stride()} is not a [rows, width] view")
+        expect *= t.size(d)
+    return (t.stride(0) if t.dim() else 1), cs
 
 def _permuted_dense(p):
     """True when `p` fills its memory exactly once in some order of its dimensions (a transposed or permuted dense tensor)"""
@@ -187,7 +259,8 @@ def prune_points(gaussians, mask):
 
 def to_fused(optimizer):
     """A FusedAdamW over the SAME parameter tensors, groups (incl. "name" and the current lr) and hyper-parameters as an existing
-    torch.optim.AdamW, carrying its state over."""
+    torch.optim.AdamW, carrying its state over.  With LGR_SELECTIVE_ADAM=1 in the environment at the time of the call, a
+    SelectiveAdamW instead (opt-in: inactive Gaussians are not stepped, so results differ from the reference's by design)."""
     if isinstance(optimizer, FusedAdamW):
         return optimizer
     if type(optimizer) is not torch.optim.AdamW:
@@ -197,7 +270,8 @@ def to_fused(optimizer):
         if g.get("amsgrad") or g.get("maximize") or g.get("capturable") or g.get("differentiable"):
             raise NotImplementedError("to_fused: amsgrad / maximize / capturable / differentiable groups are not supported")
     groups = [{k: v for k, v in g.items() if k not in skip} for g in optimizer.param_groups]
-    fused = FusedAdamW(groups, **{k: v for k, v in optimizer.defaults.items() if k not in skip})
+    cls = SelectiveAdamW if os.environ.get("LGR_SELECTIVE_ADAM", "0") == "1" else FusedAdamW
+    fused = cls(groups, **{k: v for k, v in optimizer.defaults.items() if k not in skip})
     for p, st in optimizer.state.items():
         fused.state[p] = st
     return fused

@@ -4,6 +4,7 @@ took; with LGR_TRACE=<file> set, the counters below are written to that file (JS
     render_fused_strided_rest          ... of which with a row-strided _features_rest (the distillation student)
     render_vq_resident / vq_materialize  calls that rendered a resident VQ model in place / resident models whose leaves were built
     adamw_steps / adamw_strided_params FusedAdamW.step() calls / row-strided parameters updated in place
+    adamw_selective_steps              SelectiveAdamW.step() calls
     unfused_exchange                   view-parallel backward passes that took the dense all-reduce of the unfused node
 Cost when LGR_TRACE is unset: one dict increment per call."""
 from __future__ import annotations
