@@ -9,6 +9,8 @@ try:  # render.py:22 / render_video.py:23 do `from gaussian_renderer import Gaus
 except Exception:  # reference checkout not on the path: the name is simply absent
     GaussianModel = None
 
+from lightgaussian_b200.renderer import significance_mode as _significance_mode  # noqa: E402
+_significance_mode()   # an unknown LGR_SIGNIFICANCE fails here, not at the first prune
 if _os.environ.get("LGR_SELECTIVE_ADAM", "0") == "1" and _os.environ.get("LGR_FUSED_OPTIM", "1") == "0":
     raise RuntimeError("LGR_SELECTIVE_ADAM=1 needs the fused optimizer: it cannot be combined with LGR_FUSED_OPTIM=0")
 if GaussianModel is not None and _os.environ.get("LGR_FUSED_OPTIM", "1") != "0":

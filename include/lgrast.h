@@ -161,6 +161,35 @@ int lgr_forward_vq(const lgr_view* view, int P, const lgr_vq_resident_params* pa
                    float* out_color, int32_t* gaussians_count, float* important_score, int32_t* radii,
                    int32_t* num_rendered, void* cuda_stream);
 
+/* ---- blending-weight significance (DESIGN.md section 3, "Blending-weight significance") ----
+ * The count forwards above with one more output, blend_weight[P] (int64, device, fully written: no zero-init needed):
+ *   blend_weight[i] = sum over the pixels p that blend Gaussian i in this view of rint(fl(alpha * T) * 2^32),
+ * alpha and T being the float32 alpha and pre-blend transmittance the colour uses, fl one rounding.  Resolution 2^-32; the sum is
+ * exact, so it does not depend on launch order, stream, binning mode, deterministic mode or tile culling.  Every other output is
+ * bit-identical to the sibling.  blend_weight is required when P > 0; the raw / VQ variants need count mode (gaussians_count and
+ * important_score set).  The round-1 blend kernels (lgr_set_blend_mode(1)) have no weight output: LGR_ERR_INVALID_ARG, nothing
+ * launched. */
+int lgr_forward_count_weight(const lgr_view* view, int P, int M,
+                             const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+                             const float* scales, const float* rotations, const float* cov3D_precomp,
+                             lgr_alloc_fn geometry_alloc, void* geometry_user,
+                             lgr_alloc_fn binning_alloc, void* binning_user,
+                             lgr_alloc_fn image_alloc, void* image_user,
+                             float* out_color, int32_t* gaussians_count, float* important_score, int64_t* blend_weight,
+                             int32_t* radii, int32_t* num_rendered, void* cuda_stream);
+int lgr_forward_raw_weight(const lgr_view* view, int P, int M, const lgr_raw_params* params,
+                           lgr_alloc_fn geometry_alloc, void* geometry_user,
+                           lgr_alloc_fn binning_alloc, void* binning_user,
+                           lgr_alloc_fn image_alloc, void* image_user,
+                           float* out_color, int32_t* gaussians_count, float* important_score, int64_t* blend_weight,
+                           int32_t* radii, int32_t* num_rendered, void* cuda_stream);
+int lgr_forward_vq_weight(const lgr_view* view, int P, const lgr_vq_resident_params* params,
+                          lgr_alloc_fn geometry_alloc, void* geometry_user,
+                          lgr_alloc_fn binning_alloc, void* binning_user,
+                          lgr_alloc_fn image_alloc, void* image_user,
+                          float* out_color, int32_t* gaussians_count, float* important_score, int64_t* blend_weight,
+                          int32_t* radii, int32_t* num_rendered, void* cuda_stream);
+
 int lgr_backward_raw(const lgr_view* view, int P, int M, int num_rendered, const lgr_raw_params* params,
                      const int32_t* radii, char* geometry_blob, char* binning_blob, char* image_blob,
                      const float* dL_dout_color, const lgr_raw_grads* grads, float* dL_dmeans2D, void* cuda_stream);

@@ -123,6 +123,15 @@ def load():
         lib.lgr_forward_vq.restype = i32
         lib.lgr_forward_vq.argtypes = [C.POINTER(LgrView), i32, C.POINTER(LgrVqResidentParams), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN, vp,
                                        vp, vp, vp, vp, C.POINTER(C.c_int32), vp]
+        # the *_weight forwards: their sibling's arguments with int64_t* blend_weight behind important_score
+        lib.lgr_forward_count_weight.restype = i32
+        lib.lgr_forward_count_weight.argtypes = fwd_common + [vp, vp, vp, vp, vp, C.POINTER(C.c_int32), vp]
+        lib.lgr_forward_raw_weight.restype = i32
+        lib.lgr_forward_raw_weight.argtypes = [C.POINTER(LgrView), i32, i32, C.POINTER(LgrRawParams), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN,
+                                               vp, vp, vp, vp, vp, vp, C.POINTER(C.c_int32), vp]
+        lib.lgr_forward_vq_weight.restype = i32
+        lib.lgr_forward_vq_weight.argtypes = [C.POINTER(LgrView), i32, C.POINTER(LgrVqResidentParams), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN,
+                                              vp, vp, vp, vp, vp, vp, C.POINTER(C.c_int32), vp]
         lib.lgr_backward_raw.restype = i32
         lib.lgr_backward_raw.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
                                          C.POINTER(LgrRawGrads), vp, vp]

@@ -168,15 +168,20 @@ __device__ __forceinline__ void ring_init(BlendRing& r, int consumers)
 // K4/K5 forward
 // ------------------------------------------------------------------------------------------------
 // PERM (deterministic mode): word 10 of each stored record is the instance's unsorted index perm[pos], which the deterministic
-// backward uses to address its per-instance partial rows
-template <bool COUNT, bool STORE, bool PERM = false>
+// backward uses to address its per-instance partial rows.
+// WEIGHT (count mode only): also weight[i] += sum over the pixels that blend Gaussian i of q = rint(fl(alpha*T) * 2^32), alpha*T
+// being the share of the pixel's colour the Gaussian supplies (DESIGN section 3, "Blending-weight significance").  q < 0.99*2^32
+// fits 32 bits; the warp sums each 16-bit half with REDUX (< 2^21, exact) and lane 0 adds them with one 64-bit integer atomic, so the
+// per-view sums are exact and independent of every ordering.
+template <bool COUNT, bool STORE, bool PERM = false, bool WEIGHT = false>
 __global__ void __launch_bounds__(BL_THREADS)
 blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H, int tiles_x,
                           const float2* __restrict__ means2D, const float4* __restrict__ conic_opacity, const float4* __restrict__ rgb,
                           const float* __restrict__ bg, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
                           float* __restrict__ out_color, int* __restrict__ count, float* __restrict__ rec_out, const int* __restrict__ header,
-                          const uint32_t* __restrict__ perm = nullptr)
+                          const uint32_t* __restrict__ perm = nullptr, unsigned long long* __restrict__ weight = nullptr)
 {
+    static_assert(!WEIGHT || COUNT, "the blending weight is a count-mode output");
     if (header[HDR_OVERFLOW]) return;   // the binning blob was too small for this view: the host repeats scatter + blend (lgr_bin.cuh)
     __shared__ __align__(128) BlendRing ring;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -268,6 +273,7 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
                 const float dx = LGR_SUB(q0.x, pxf), dy = LGR_SUB(q0.y, pyf);
                 const float power = lgr::pair_power(dx, dy, q0.z, q0.w, q1.x);
                 bool contrib = false;
+                uint32_t q = 0;   // WEIGHT: this lane's fixed-point alpha*T (0 when it does not blend the Gaussian)
                 if (!(power > 0.0f)) {
                     const float alpha = fminf(0.99f, LGR_MUL(q1.y, expf(power)));
                     if (!(alpha < 1.0f / 255.0f)) {
@@ -279,6 +285,7 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
                             C0 = LGR_FMA(T, LGR_MUL(alpha, q1.z), C0);
                             C1 = LGR_FMA(T, LGR_MUL(alpha, q1.w), C1);
                             C2 = LGR_FMA(T, LGR_MUL(alpha, b), C2);
+                            if (WEIGHT) q = __float2uint_rn(__fmul_rn(__fmul_rn(alpha, T), 4294967296.0f));   // 2^32: exact scaling
                             T = test_T;
                             last = pos_base + (uint32_t)j;
                             contrib = true;
@@ -288,6 +295,10 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
                 if (COUNT) {
                     const unsigned cm = __ballot_sync(FULL, contrib);
                     if (cm != 0 && lane == 0) atomicAdd(&count[__float_as_uint(r[9])], __popc(cm));
+                    if (WEIGHT && cm != 0) {
+                        const unsigned lo = __reduce_add_sync(FULL, q & 0xffffu), hi = __reduce_add_sync(FULL, q >> 16);
+                        if (lane == 0) atomicAdd(&weight[__float_as_uint(r[9])], ((unsigned long long)hi << 16) + lo);
+                    }
                 }
                 if (__all_sync(FULL, T < 0.f)) break;
             }

@@ -1155,7 +1155,7 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
                  lgr_alloc_fn geometry_alloc, void* geometry_user, lgr_alloc_fn binning_alloc, void* binning_user,
                  lgr_alloc_fn image_alloc, void* image_user, float* out_color, int32_t* gaussians_count, float* important_score,
                  int32_t* radii, int32_t* num_rendered, void* cuda_stream, bool count_mode, const lgr_raw_params* raw = nullptr,
-                 const lgr_vq_resident_params* vq = nullptr)
+                 const lgr_vq_resident_params* vq = nullptr, int64_t* blend_weight = nullptr)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     if (vq) {  // resident VQ model: attributes and colour rows come from the compressed arrays (validated by lgr_forward_vq)
@@ -1207,6 +1207,11 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
         }
     }
     if (g_det && !det_supported("lgr_forward")) return LGR_ERR_INVALID_ARG;
+    if (blend_weight && (!count_mode || g_blend_mode != 0)) {
+        g_last_error = g_blend_mode != 0 ? "lgr_forward_*_weight: the blending weight needs the ring blend kernels; lgr_set_blend_mode(1) has no weight output"
+                                         : "lgr_forward_*_weight: the blending weight is a count-mode output";
+        return LGR_ERR_INVALID_ARG;
+    }
     const bool debug = v->debug != 0;
     *num_rendered = 0;
     const int gx = (W + LGR_TILE - 1) / LGR_TILE, gy = (H + LGR_TILE - 1) / LGR_TILE;
@@ -1276,8 +1281,13 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
     // K4/K5 -- and everything of it that has to be repeated when the binning blob turns out too small
     auto launch_blend = [&]() -> int {
         if (count_mode) LGR_CUDA_TRY(cudaMemsetAsync(gaussians_count, 0, sizeof(int) * (size_t)P, stream));
+        if (blend_weight) LGR_CUDA_TRY(cudaMemsetAsync(blend_weight, 0, sizeof(int64_t) * (size_t)P, stream));
         ProfScope ps(count_mode ? ST_BLEND_FWD_COUNT : ST_BLEND_FWD, stream);
-        if (g_blend_mode == 0 && count_mode)
+        if (blend_weight)   // refused above unless g_blend_mode == 0 and count_mode
+            blend_forward_ring_kernel<true, false, false, true><<<tiles, BL_THREADS, 0, stream>>>(
+                img.ranges, bin.point_list, W, H, gx, geo.means2D, geo.conic_opacity, geo.rgb, v->background, img.final_T, img.n_contrib,
+                out_color, gaussians_count, nullptr, geo.num_rendered, nullptr, reinterpret_cast<unsigned long long*>(blend_weight));
+        else if (g_blend_mode == 0 && count_mode)
             blend_forward_ring_kernel<true, false><<<tiles, BL_THREADS, 0, stream>>>(img.ranges, bin.point_list, W, H, gx, geo.means2D, geo.conic_opacity,
                                                                                       geo.rgb, v->background, img.final_T, img.n_contrib, out_color,
                                                                                       gaussians_count, nullptr, geo.num_rendered);
@@ -1647,6 +1657,28 @@ int lgr_forward_count(const lgr_view* view, int P, int M, const float* means3D, 
                         important_score, radii, num_rendered, cuda_stream, true);
 }
 
+// the *_weight entry points: their sibling's contract plus blend_weight [P], which they require
+static bool weight_present(const char* what, int P, const int64_t* blend_weight)
+{
+    if (P > 0 && !blend_weight) {
+        g_last_error = std::string(what) + ": blend_weight missing";
+        return false;
+    }
+    return true;
+}
+
+int lgr_forward_count_weight(const lgr_view* view, int P, int M, const float* means3D, const float* shs, const float* colors_precomp,
+                             const float* opacities, const float* scales, const float* rotations, const float* cov3D_precomp,
+                             lgr_alloc_fn geometry_alloc, void* geometry_user, lgr_alloc_fn binning_alloc, void* binning_user,
+                             lgr_alloc_fn image_alloc, void* image_user, float* out_color, int32_t* gaussians_count, float* important_score,
+                             int64_t* blend_weight, int32_t* radii, int32_t* num_rendered, void* cuda_stream)
+{
+    if (!weight_present("lgr_forward_count_weight", P, blend_weight)) return LGR_ERR_INVALID_ARG;
+    return forward_impl(view, P, M, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, geometry_alloc,
+                        geometry_user, binning_alloc, binning_user, image_alloc, image_user, out_color, gaussians_count,
+                        important_score, radii, num_rendered, cuda_stream, true, nullptr, nullptr, blend_weight);
+}
+
 int lgr_backward(const lgr_view* v, int P, int M, int num_rendered, const float* means3D, const float* shs,
                  const float* colors_precomp, const float* scales, const float* rotations, const float* cov3D_precomp,
                  const int32_t* radii, char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color,
@@ -1713,9 +1745,10 @@ int lgr_backward(const lgr_view* v, int P, int M, int num_rendered, const float*
     return LGR_OK;
 }
 
-int lgr_forward_raw(const lgr_view* view, int P, int M, const lgr_raw_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
-                    lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
-                    int32_t* gaussians_count, float* important_score, int32_t* radii, int32_t* num_rendered, void* cuda_stream)
+static int forward_raw_impl(const lgr_view* view, int P, int M, const lgr_raw_params* params, lgr_alloc_fn geometry_alloc,
+                            void* geometry_user, lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user,
+                            float* out_color, int32_t* gaussians_count, float* important_score, int64_t* blend_weight, int32_t* radii,
+                            int32_t* num_rendered, void* cuda_stream)
 {
     if (!params || M < 1) {
         g_last_error = "lgr_forward_raw: params missing or M < 1";
@@ -1724,12 +1757,31 @@ int lgr_forward_raw(const lgr_view* view, int P, int M, const lgr_raw_params* pa
     const bool count_mode = gaussians_count != nullptr;
     return forward_impl(view, P, M, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, geometry_alloc, geometry_user,
                         binning_alloc, binning_user, image_alloc, image_user, out_color, gaussians_count, important_score, radii,
-                        num_rendered, cuda_stream, count_mode, params);
+                        num_rendered, cuda_stream, count_mode, params, nullptr, blend_weight);
 }
 
-int lgr_forward_vq(const lgr_view* view, int P, const lgr_vq_resident_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
-                   lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
-                   int32_t* gaussians_count, float* important_score, int32_t* radii, int32_t* num_rendered, void* cuda_stream)
+int lgr_forward_raw(const lgr_view* view, int P, int M, const lgr_raw_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
+                    lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
+                    int32_t* gaussians_count, float* important_score, int32_t* radii, int32_t* num_rendered, void* cuda_stream)
+{
+    return forward_raw_impl(view, P, M, params, geometry_alloc, geometry_user, binning_alloc, binning_user, image_alloc, image_user, out_color,
+                            gaussians_count, important_score, nullptr, radii, num_rendered, cuda_stream);
+}
+
+int lgr_forward_raw_weight(const lgr_view* view, int P, int M, const lgr_raw_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
+                           lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
+                           int32_t* gaussians_count, float* important_score, int64_t* blend_weight, int32_t* radii, int32_t* num_rendered,
+                           void* cuda_stream)
+{
+    if (!weight_present("lgr_forward_raw_weight", P, blend_weight)) return LGR_ERR_INVALID_ARG;
+    return forward_raw_impl(view, P, M, params, geometry_alloc, geometry_user, binning_alloc, binning_user, image_alloc, image_user, out_color,
+                            gaussians_count, important_score, blend_weight, radii, num_rendered, cuda_stream);
+}
+
+static int forward_vq_impl(const lgr_view* view, int P, const lgr_vq_resident_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
+                           lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
+                           int32_t* gaussians_count, float* important_score, int64_t* blend_weight, int32_t* radii, int32_t* num_rendered,
+                           void* cuda_stream)
 {
     const lgr_vq_resident_params* q = params;
     if (!q || q->D < 3 || q->D % 3 != 0 || q->D > 48 || q->Dp < q->D || q->Dp % 8 != 0 || q->K < 1) {
@@ -1767,7 +1819,25 @@ int lgr_forward_vq(const lgr_view* view, int P, const lgr_vq_resident_params* pa
     }
     return forward_impl(view, P, M, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, geometry_alloc, geometry_user,
                         binning_alloc, binning_user, image_alloc, image_user, out_color, gaussians_count, important_score, radii,
-                        num_rendered, cuda_stream, gaussians_count != nullptr, nullptr, q);
+                        num_rendered, cuda_stream, gaussians_count != nullptr, nullptr, q, blend_weight);
+}
+
+int lgr_forward_vq(const lgr_view* view, int P, const lgr_vq_resident_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
+                   lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
+                   int32_t* gaussians_count, float* important_score, int32_t* radii, int32_t* num_rendered, void* cuda_stream)
+{
+    return forward_vq_impl(view, P, params, geometry_alloc, geometry_user, binning_alloc, binning_user, image_alloc, image_user, out_color,
+                           gaussians_count, important_score, nullptr, radii, num_rendered, cuda_stream);
+}
+
+int lgr_forward_vq_weight(const lgr_view* view, int P, const lgr_vq_resident_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
+                          lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
+                          int32_t* gaussians_count, float* important_score, int64_t* blend_weight, int32_t* radii, int32_t* num_rendered,
+                          void* cuda_stream)
+{
+    if (!weight_present("lgr_forward_vq_weight", P, blend_weight)) return LGR_ERR_INVALID_ARG;
+    return forward_vq_impl(view, P, params, geometry_alloc, geometry_user, binning_alloc, binning_user, image_alloc, image_user, out_color,
+                           gaussians_count, important_score, blend_weight, radii, num_rendered, cuda_stream);
 }
 
 // lgr_backward_raw (one call for both stages, dense outputs) asks stage 1 to clear the gradient rows from inside the blend backward

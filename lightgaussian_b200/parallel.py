@@ -99,18 +99,45 @@ def allreduce_counts(count: torch.Tensor, world: int) -> torch.Tensor:
     return c
 
 
+# the int64 sum of the fixed-point blending weights cannot overflow below this many pixel-views: each pixel adds at most 0.99 * 2^32
+WEIGHT_PIXEL_VIEWS_MAX = 2 ** 31
+
+
+def check_weight_bound(cameras) -> int:
+    """Pixel-views of `cameras` (sum of W * H); raises before anything runs when their blending weights could overflow int64."""
+    n = sum(int(c.image_width) * int(c.image_height) for c in cameras)
+    if n >= WEIGHT_PIXEL_VIEWS_MAX:
+        raise RuntimeError(f"blend_weight significance: {n} pixel-views over {len(cameras)} cameras; the exact int64 sum is only "
+                           f"guaranteed below 2^31 pixel-views (about 1000 views at 1080p)")
+    return n
+
+
 def sharded_prune_list(gaussians, cameras, pipe, background, count_render_fn, rank: int = 0, world: int = 1):
     """prune.prune_list (reference prune.py:133-157) with the camera loop partitioned over ranks.
     Returns (gaussian_list int64[P], imp_list float32[P]) identical on every rank and for every world size:
     counts are summed as integers, and the score is opacity * total count (opacity does not change inside
-    the loop -- there is no optimizer step in prune_list)."""
-    total = None
+    the loop -- there is no optimizer step in prune_list).
+    With LGR_SIGNIFICANCE=blend_weight, imp_list is the total blending weight instead: each view's int64 `blend_weight_fx` is
+    summed as integers, all-reduced once next to the counts, and converted to float32 once, so it is as partition-independent."""
+    from .renderer import significance_mode, weight_score
+    weight = significance_mode() == "blend_weight"
+    if weight:
+        check_weight_bound(cameras)
+    total = wtotal = None
     for i in shard_views(len(cameras), rank, world):
         pkg = count_render_fn(cameras[i], gaussians, pipe, background)
         c = pkg["gaussians_count"].to(torch.int64)
         total = c if total is None else total + c
+        if weight:
+            w = pkg["blend_weight_fx"].to(torch.int64)
+            wtotal = w if wtotal is None else wtotal + w
     if total is None:
         total = torch.zeros(gaussians.get_xyz.shape[0], dtype=torch.int64, device=gaussians.get_xyz.device)
+    if weight:
+        if wtotal is None:
+            wtotal = torch.zeros_like(total)
+        both = allreduce_counts(torch.stack([total, wtotal]), world)
+        return both[0], weight_score(both[1])
     total = allreduce_counts(total, world)
     imp = gaussians.get_opacity.detach().reshape(-1) * total.to(torch.float32)
     return total, imp

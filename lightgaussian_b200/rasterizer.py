@@ -80,8 +80,21 @@ def _make_view(device, background, viewmatrix, projmatrix, campos, tan_fovx, tan
     return v, keep
 
 
+def _weight_out(count_mode, blend_weight, P, device):
+    """The int64 [P] blending-weight output a count forward was given, checked (None when there is none)."""
+    if blend_weight is None:
+        return None
+    if not count_mode:
+        raise RuntimeError("blend_weight is a count-mode output")
+    if blend_weight.dtype != torch.int64 or tuple(blend_weight.shape) != (P,) or not blend_weight.is_contiguous() or blend_weight.device != device:
+        raise RuntimeError(f"blend_weight must be a contiguous int64 [{P}] tensor on {device}")
+    return blend_weight
+
+
 def _forward_native(count_mode, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
-                    projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug):
+                    projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug, blend_weight=None):
+    """blend_weight: optional int64 [P] output of a count forward, overwritten with this view's fixed-point blending weights
+    (lgr_forward_count_weight)."""
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:68-70
     lib = capi.load()
@@ -99,6 +112,7 @@ def _forward_native(count_mode, background, means3D, colors, opacity, scales, ro
     if count_mode:
         count = torch.empty((P,), dtype=torch.int32, device=device)
         score = torch.empty((P,), dtype=torch.float32, device=device)
+    weight = _weight_out(count_mode, blend_weight, P, device)
     _apply_deterministic_mode()
     slots = [capi.BlobSlot(device) for _ in range(3)]
     num_rendered = C.c_int32(0)
@@ -110,12 +124,15 @@ def _forward_native(count_mode, background, means3D, colors, opacity, scales, ro
             common = (C.byref(view), P, M, capi.ptr(means3D_c), capi.ptr(sh_c), capi.ptr(colors_c), capi.ptr(opacity_c),
                       capi.ptr(scales_c), capi.ptr(rot_c), capi.ptr(cov_c),
                       capi.ALLOC_CB, slots[0].key, capi.ALLOC_CB, slots[1].key, capi.ALLOC_CB, slots[2].key)
-            if count_mode:
+            if weight is not None:
+                st = lib.lgr_forward_count_weight(*common, out_color.data_ptr(), capi.ptr(count), capi.ptr(score), capi.ptr(weight),
+                                                  capi.ptr(radii), C.byref(num_rendered), stream)
+            elif count_mode:
                 st = lib.lgr_forward_count(*common, out_color.data_ptr(), capi.ptr(count), capi.ptr(score), capi.ptr(radii),
                                            C.byref(num_rendered), stream)
             else:
                 st = lib.lgr_forward(*common, out_color.data_ptr(), capi.ptr(radii), C.byref(num_rendered), stream)
-        capi.check(st, "lgr_forward_count" if count_mode else "lgr_forward")
+        capi.check(st, "lgr_forward_count_weight" if weight is not None else "lgr_forward_count" if count_mode else "lgr_forward")
     finally:
         for s in slots:
             s.release()
@@ -139,9 +156,12 @@ class _NativeModule:
 
     @staticmethod
     def count_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
-                        projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug, f_count=True):
+                        projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug, f_count=True,
+                        blend_weight=None):
+        """The reference's tuple; blend_weight (int64 [P], optional) also receives the view's fixed-point blending weights."""
         return _forward_native(True, background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
-                               projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug)
+                               projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug,
+                               blend_weight)
 
     @staticmethod
     def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
@@ -233,18 +253,22 @@ class _RasterizeGaussians(torch.autograd.Function):
                 fit(grad_scales, scales), fit(grad_rotations, rotations), fit(grad_cov3Ds_precomp, cov3Ds_precomp), None)
 
     @staticmethod
-    def forward_count(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+    def forward_count(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, blend_weight=None):
         """No autograd, exactly like the reference (:140-189)."""
         assert raster_settings.f_count
         args = _pack_args(raster_settings, means3D, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, sh)
-        gaussians_count, important_score, _, color, radii, _, _, _ = _C.count_gaussians(*args, raster_settings.f_count)
+        gaussians_count, important_score, _, color, radii, _, _, _ = _C.count_gaussians(*args, raster_settings.f_count,
+                                                                                        blend_weight=blend_weight)
         return gaussians_count, important_score, color, radii
 
 
-def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                        blend_weight=None):
     if raster_settings.f_count:
         return _RasterizeGaussians.forward_count(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                                 raster_settings)
+                                                 raster_settings, blend_weight)
+    if blend_weight is not None:
+        raise RuntimeError("blend_weight is a count-mode output (raster_settings.f_count)")
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings)
 
 
@@ -258,7 +282,7 @@ class GaussianRasterizer(nn.Module):
             rs = self.raster_settings
             return _C.mark_visible(positions, rs.viewmatrix, rs.projmatrix)
 
-    def _run(self, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp):
+    def _run(self, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, blend_weight=None):
         if (shs is None) == (colors_precomp is None):
             raise Exception("Please provide excatly one of either SHs or precomputed colors!")
         has_sr = scales is not None or rotations is not None
@@ -271,14 +295,16 @@ class GaussianRasterizer(nn.Module):
         rotations = absent if rotations is None else rotations
         cov3D_precomp = absent if cov3D_precomp is None else cov3D_precomp
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   self.raster_settings)
+                                   self.raster_settings, blend_weight)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None):
         return self._run(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp)
 
     def forward_count(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                      cov3D_precomp=None):
-        return self._run(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp)
+                      cov3D_precomp=None, blend_weight=None):
+        """blend_weight: optional int64 [P] tensor that receives this view's fixed-point blending weights (include/lgrast.h,
+        lgr_forward_count_weight); the four outputs are unchanged."""
+        return self._run(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, blend_weight)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -311,7 +337,8 @@ def _raw_struct(xyz, dc, rest, scaling, rotation, opacity):
                              0 if dense else rest_row_stride(rest))
 
 
-def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacity):
+def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacity, blend_weight=None):
+    """blend_weight: optional int64 [P] output of a count forward (lgr_forward_raw_weight), as in _forward_native."""
     lib = capi.load()
     device = xyz.device
     P, H, W = xyz.size(0), int(rs.image_height), int(rs.image_width)
@@ -329,6 +356,7 @@ def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacit
     if count_mode:
         count = torch.empty((P,), dtype=torch.int32, device=device)
         score = torch.empty((P,), dtype=torch.float32, device=device)
+    weight = _weight_out(count_mode, blend_weight, P, device)
     _apply_deterministic_mode()
     slots = [capi.BlobSlot(device) for _ in range(3)]
     num_rendered = C.c_int32(0)
@@ -337,10 +365,14 @@ def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacit
             view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W, rs.scale_modifier,
                                     rs.sh_degree, rs.prefiltered, rs.debug)
             params = _raw_struct(*leaves)
-            st = lib.lgr_forward_raw(C.byref(view), P, M, C.byref(params), capi.ALLOC_CB, slots[0].key, capi.ALLOC_CB, slots[1].key,
-                                     capi.ALLOC_CB, slots[2].key, out_color.data_ptr(), capi.ptr(count), capi.ptr(score), capi.ptr(radii),
-                                     C.byref(num_rendered), capi.current_stream_ptr(device))
-        capi.check(st, "lgr_forward_raw")
+            head = (C.byref(view), P, M, C.byref(params), capi.ALLOC_CB, slots[0].key, capi.ALLOC_CB, slots[1].key, capi.ALLOC_CB, slots[2].key,
+                    out_color.data_ptr(), capi.ptr(count), capi.ptr(score))
+            tail = (capi.ptr(radii), C.byref(num_rendered), capi.current_stream_ptr(device))
+            if weight is not None:
+                st = lib.lgr_forward_raw_weight(*head, capi.ptr(weight), *tail)
+            else:
+                st = lib.lgr_forward_raw(*head, *tail)
+        capi.check(st, "lgr_forward_raw_weight" if weight is not None else "lgr_forward_raw")
     finally:
         for s_ in slots:
             s_.release()
@@ -352,9 +384,10 @@ def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacit
     return count, score, int(num_rendered.value), out_color, radii, geom, binning, img, leaves
 
 
-def forward_vq_native(count_mode, rs, xyz, store):
+def forward_vq_native(count_mode, rs, xyz, store, blend_weight=None):
     """Forward of a resident VQ model (lgr_forward_vq): (count, score, color, radii), count and score None unless count_mode.
-    `store` is a vqresident.ResidentVQ; `xyz` its positions ([P,3] float32, the model's _xyz).  No autograd."""
+    `store` is a vqresident.ResidentVQ; `xyz` its positions ([P,3] float32, the model's _xyz).  No autograd.
+    blend_weight: optional int64 [P] output of a count forward (lgr_forward_vq_weight), as in _forward_native."""
     lib = capi.load()
     arrays = (xyz, store.attr, store.slot, store.codebook, store.nonvq)
     if not all(t.is_cuda and t.device == xyz.device and t.is_contiguous() for t in arrays):
@@ -369,6 +402,7 @@ def forward_vq_native(count_mode, rs, xyz, store):
     if count_mode:
         count = torch.empty((P,), dtype=torch.int32, device=device)
         score = torch.empty((P,), dtype=torch.float32, device=device)
+    weight = _weight_out(count_mode, blend_weight, P, device)
     params = capi.LgrVqResidentParams(capi.ptr(xyz), capi.ptr(store.attr), capi.ptr(store.slot), capi.ptr(store.codebook),
                                       capi.ptr(store.nonvq), int(store.attr.dtype == torch.float16),
                                       int(store.nonvq.dtype == torch.float16), store.D, store.Dp, store.K)
@@ -379,10 +413,14 @@ def forward_vq_native(count_mode, rs, xyz, store):
         with torch.cuda.device(device):
             view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W, rs.scale_modifier,
                                     rs.sh_degree, rs.prefiltered, rs.debug)
-            st = lib.lgr_forward_vq(C.byref(view), P, C.byref(params), capi.ALLOC_CB, slots[0].key, capi.ALLOC_CB, slots[1].key,
-                                    capi.ALLOC_CB, slots[2].key, out_color.data_ptr(), capi.ptr(count), capi.ptr(score), capi.ptr(radii),
-                                    C.byref(num_rendered), capi.current_stream_ptr(device))
-        capi.check(st, "lgr_forward_vq")
+            head = (C.byref(view), P, C.byref(params), capi.ALLOC_CB, slots[0].key, capi.ALLOC_CB, slots[1].key, capi.ALLOC_CB, slots[2].key,
+                    out_color.data_ptr(), capi.ptr(count), capi.ptr(score))
+            tail = (capi.ptr(radii), C.byref(num_rendered), capi.current_stream_ptr(device))
+            if weight is not None:
+                st = lib.lgr_forward_vq_weight(*head, capi.ptr(weight), *tail)
+            else:
+                st = lib.lgr_forward_vq(*head, *tail)
+        capi.check(st, "lgr_forward_vq_weight" if weight is not None else "lgr_forward_vq")
     finally:
         for s_ in slots:
             s_.release()
@@ -906,13 +944,15 @@ def sh_grad_from_views(xyz, campos_all, d_rgb_all, dc_like, rest_like, sh_degree
     return d_dc, d_rest
 
 
-def rasterize_raw_leaves(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity, raster_settings):
+def rasterize_raw_leaves(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity, raster_settings, blend_weight=None):
     """(color, radii) or, in count mode, (gaussians_count, important_score, color, radii) -- same as rasterize_gaussians."""
     if raster_settings.f_count:
         count, score, _, color, radii, _, _, _, _ = _forward_raw_native(True, raster_settings, xyz.detach(), features_dc.detach(),
                                                                         features_rest.detach(), scaling.detach(), rotation.detach(),
-                                                                        opacity.detach())
+                                                                        opacity.detach(), blend_weight)
         return count, score, color, radii
+    if blend_weight is not None:
+        raise RuntimeError("blend_weight is a count-mode output (raster_settings.f_count)")
     return _RasterizeRawLeaves.apply(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity, raster_settings)
 
 

@@ -23,6 +23,22 @@ from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rast
 
 _LEAVES = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
 
+SIGNIFICANCE_MODES = ("count", "blend_weight")
+WEIGHT_SCALE = 2.0 ** -32   # resolution of the fixed-point blending weight (include/lgrast.h, lgr_forward_count_weight)
+
+
+def significance_mode() -> str:
+    """LGR_SIGNIFICANCE, read at call time: "count" (unset; the reference's opacity * count) or "blend_weight" (sum of alpha * T)."""
+    mode = os.environ.get("LGR_SIGNIFICANCE", "count")
+    if mode not in SIGNIFICANCE_MODES:
+        raise RuntimeError(f"LGR_SIGNIFICANCE={mode!r}: expected one of {', '.join(SIGNIFICANCE_MODES)}")
+    return mode
+
+
+def weight_score(blend_weight_fx: torch.Tensor) -> torch.Tensor:
+    """float32 score of int64 fixed-point blending weights: float32(float64(fx) * 2^-32)."""
+    return (blend_weight_fx.to(torch.float64) * WEIGHT_SCALE).to(torch.float32)
+
 
 def _can_fuse(pc, pipe, override_color) -> bool:
     """The fused path needs GaussianModel-style raw leaves with the standard activations
@@ -100,8 +116,10 @@ def eval_sh_torch(deg: int, sh: torch.Tensor, dirs: torch.Tensor) -> torch.Tenso
     return out
 
 
-def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, f_count):
+def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, f_count, weight=False):
     xyz = pc.get_xyz
+    # weight: count mode that also returns the view's fixed-point blending weights (int64 [P], fully written by the forward)
+    blend_weight = torch.empty((xyz.shape[0],), dtype=torch.int64, device=xyz.device) if weight else None
     # grad placeholder for the screen-space means, as the reference builds it (:37-46)
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
     try:
@@ -127,15 +145,15 @@ def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_col
     store = _resident_store(pc, pipe, override_color)
     if store is not None:
         trace.bump("render_vq_resident")
-        count, score, color, radii = forward_vq_native(f_count, settings, pc._xyz.detach(), store)
-        return _package((count, score, color, radii) if f_count else (color, radii), screenspace_points, f_count)
+        count, score, color, radii = forward_vq_native(f_count, settings, pc._xyz.detach(), store, blend_weight)
+        return _package((count, score, color, radii) if f_count else (color, radii), screenspace_points, f_count, blend_weight)
     if _can_fuse(pc, pipe, override_color):
         trace.bump("render_fused")
         if not pc._features_rest.is_contiguous():
             trace.bump("render_fused_strided_rest")
         outputs = rasterize_raw_leaves(pc._xyz, screenspace_points, pc._features_dc, pc._features_rest, pc._scaling, pc._rotation,
-                                       pc._opacity, settings)
-        return _package(outputs, screenspace_points, f_count)
+                                       pc._opacity, settings, blend_weight)
+        return _package(outputs, screenspace_points, f_count, blend_weight)
 
     trace.bump("render_unfused")
     rasterizer = GaussianRasterizer(raster_settings=settings)
@@ -158,11 +176,15 @@ def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_col
     else:
         appearance["shs"] = pc.get_features
 
-    outputs = rasterizer(means3D=xyz, means2D=screenspace_points, opacities=pc.get_opacity, **appearance, **geometry)
-    return _package(outputs, screenspace_points, f_count)
+    if blend_weight is not None:
+        outputs = rasterizer.forward_count(means3D=xyz, means2D=screenspace_points, opacities=pc.get_opacity, **appearance, **geometry,
+                                           blend_weight=blend_weight)
+    else:
+        outputs = rasterizer(means3D=xyz, means2D=screenspace_points, opacities=pc.get_opacity, **appearance, **geometry)
+    return _package(outputs, screenspace_points, f_count, blend_weight)
 
 
-def _package(outputs, screenspace_points, f_count):
+def _package(outputs, screenspace_points, f_count, blend_weight=None):
     if f_count:
         gaussians_count, important_score, rendered_image, radii = outputs
     else:
@@ -176,6 +198,9 @@ def _package(outputs, screenspace_points, f_count):
     if f_count:
         result["gaussians_count"] = gaussians_count
         result["important_score"] = important_score
+    if blend_weight is not None:
+        result["important_score"] = weight_score(blend_weight)
+        result["blend_weight_fx"] = blend_weight
     return result
 
 
@@ -185,5 +210,9 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
 
 def count_render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):
-    """render() plus per-Gaussian `gaussians_count` and `important_score` for this view (prune.py:133-157)."""
-    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, True)
+    """render() plus per-Gaussian `gaussians_count` and `important_score` for this view (prune.py:133-157).
+    With LGR_SIGNIFICANCE=blend_weight (read at each call), `important_score` is instead the Gaussian's blending weight in this view,
+    the sum of alpha * T over the pixels that blend it, and the dict gains `blend_weight_fx`, the same sums as exact int64 in units
+    of 2^-32 (DESIGN.md section 3).  `gaussians_count` is the same in both modes."""
+    weight = significance_mode() == "blend_weight"
+    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, True, weight)
