@@ -441,16 +441,19 @@ int lgr_set_blend_mode(int mode);
 
 /* Binning (per-tile depth-ordered instance lists; replaces the scan + 64-bit radix sort of RAST/cuda_rasterizer/rasterizer_impl.cu:278-319
  * and its blocking device-to-host copy of num_rendered at :282).  2 (default) = depth sort of the P Gaussians + stable tile bucketing with the
- * CUDA toolkit's radix sort / scan, one stream synchronisation for the instance count (one binning_alloc call, the reference's behaviour).
- * 0 = hand-written kernels (csrc/lgr_bin.cuh), no library and no GPU idle on the host: the binning allocator is called BEFORE the instance
- * count is known, with a size from a running estimate; the kernels bound their stores by that capacity, the host reads the count while the
- * blend kernel is already running and repeats scatter + blend with an exactly sized blob (a second binning_alloc call) when the estimate was
- * too small.  1 = the same kernels, blob sized exactly after a stream synchronisation.  All three produce bit-identical lists
- * (tests/test_gpu_binning.py); 2 is the default because it is the fastest measured (DESIGN.md section 9); it is also used automatically above
- * 32 768 tiles.  Process-wide.  lgr_binning_overflows() = views that took the repeat. */
+ * CUDA toolkit's radix sort / scan, no GPU idle on the host: the binning allocator is called BEFORE the instance count is known, with a size
+ * from a running estimate (25 % above the previous view); emit, tile sort and ranges run over that capacity (the slots past the count hold a
+ * pad key that sorts after every tile), the host reads the count while the blend kernel is already queued and repeats emit, sort, ranges and
+ * blend with an exactly sized blob (a second binning_alloc call) when the estimate was too small.  Deterministic mode, or the environment
+ * variable LGR_BINNING_SYNC=1, sizes the blob exactly after one stream synchronisation instead (one binning_alloc call, the reference's
+ * behaviour).  0 = hand-written kernels (csrc/lgr_bin.cuh), no library, the same estimate and repeat.  1 = the same kernels, blob sized
+ * exactly after a stream synchronisation.  All three produce bit-identical lists (tests/test_gpu_binning.py); 2 is the default because it is
+ * the fastest measured (DESIGN.md section 9); it is also used automatically above 32 768 tiles.  Process-wide.
+ * lgr_binning_overflows() = views that took the repeat; lgr_forward_stream_syncs() = forwards that synchronised the stream for the count. */
 int lgr_set_binning_mode(int mode);
 uint64_t lgr_binning_overflows(void);
-void lgr_set_binning_estimate(uint64_t instances);   /* overwrite the running estimate of mode 0 (tests; 0 = forget) */
+uint64_t lgr_forward_stream_syncs(void);
+void lgr_set_binning_estimate(uint64_t instances);   /* overwrite the running estimate of modes 0 and 2 (tests; 0 = forget) */
 
 /* Deterministic mode (default off).  On: every output is a function of the inputs alone, whatever the block scheduling, the stream or
  * other work on the GPU.  The blend backward writes one partial row per (tile, Gaussian) instance, summing the 8 warps of a tile in warp

@@ -220,6 +220,7 @@ def load():
         lib.lgr_last_error.restype = C.c_char_p
         lib.lgr_launch_count.restype = C.c_uint64
         lib.lgr_binning_overflows.restype = C.c_uint64
+        lib.lgr_forward_stream_syncs.restype = C.c_uint64
         lib.lgr_set_binning_estimate.restype = None
         lib.lgr_set_binning_estimate.argtypes = [C.c_uint64]
         for name in ("lgr_geometry_layout", "lgr_image_layout", "lgr_binning_layout"):
@@ -324,14 +325,20 @@ DEFAULT_BINNING_MODE = 2
 
 
 def set_binning_mode(mode: int) -> None:
-    """2 = library radix sorts + scan (default, fastest measured), 0 = hand-written binning kernels with an estimated blob size
-    (no library, no GPU idle on the host), 1 = the same with an exact size (one stream sync)"""
+    """2 = library radix sorts + scan (default, fastest measured), 0 = hand-written binning kernels (no library); both size the
+    binning blob from an estimate (no GPU idle on the host), 1 = hand-written kernels with an exact size (one stream sync)"""
     check(load().lgr_set_binning_mode(int(mode)), "lgr_set_binning_mode")
 
 
 def binning_overflows() -> int:
-    """views whose binning blob estimate was too small (scatter + blend repeated) since load"""
+    """views whose binning blob estimate was too small (binning + blend repeated) since load"""
     return int(load().lgr_binning_overflows())
+
+
+def forward_stream_syncs() -> int:
+    """forwards that synchronised the stream to size the binning blob exactly since load (deterministic mode, binning mode 1,
+    LGR_BINNING_SYNC=1); the default forward takes none"""
+    return int(load().lgr_forward_stream_syncs())
 
 
 def set_vq_mode(mode: int) -> None:
@@ -356,7 +363,7 @@ def set_kback_mode(mode: int) -> None:
 
 
 def set_binning_estimate(instances: int) -> None:
-    """overwrite the running instance estimate of binning mode 0 (tests; 0 = forget it)"""
+    """overwrite the running instance estimate of binning modes 0 and 2 (tests; 0 = forget it)"""
     load().lgr_set_binning_estimate(C.c_uint64(int(instances)))
 
 

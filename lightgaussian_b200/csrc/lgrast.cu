@@ -27,7 +27,9 @@
 #include <cmath>
 #include <algorithm>
 #include <atomic>
+#include <climits>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -48,12 +50,12 @@ constexpr int DET_ROW = 9;      // floats per partial row of the deterministic b
 
 thread_local std::string g_last_error;
 int g_blend_mode = 0;   // 0 = ring kernels (lgr_blend.cuh), 1 = round-1 kernels (kept for A/B measurements and as a cross-check in the tests)
-// binning: 2 = library radix sorts + scan with one host synchronisation for the instance count (default: the fastest path measured,
-// 0.50 ms per view at 3M / 1080p); 0 = hand-written kernels (lgr_bin.cuh), binning blob sized from a running estimate, no GPU idle on the
-// host (0.76 ms: correct and library-free, but its serial tile-ranking warp is slower than two library radix passes -- DESIGN.md section 9);
-// 1 = hand-written kernels, blob sized exactly after a stream synchronisation
+// binning: 2 = library radix sorts + scan, binning blob sized from a running estimate, no GPU idle on the host (default: the fastest path
+// measured, DESIGN.md section 4; deterministic mode sizes the blob exactly after a host synchronisation); 0 = hand-written kernels
+// (lgr_bin.cuh), the same estimate (0.76 ms: correct and library-free, but its serial tile-ranking warp is slower than two library radix
+// passes -- DESIGN.md section 9); 1 = hand-written kernels, blob sized exactly after a stream synchronisation
 int g_bin_mode = 2;
-std::atomic<size_t> g_bin_hint{0};   // running estimate of the listed instances per view (mode 0)
+std::atomic<size_t> g_bin_hint{0};   // running estimate of the listed instances per view (modes 0 and 2)
 int g_vq_mode = 0;      // VecTree nearest-code search: 0 = tensor-core coarse pass + exact FP32 rescore (d <= 32), 1 = FP32 FFMA kernel only
 // deterministic mode (lgr_set_deterministic): fixed-order reductions in place of the float atomics of the blend backward and the VecTree
 // accumulation; needs library binning and the ring blend kernels
@@ -259,11 +261,12 @@ ImageState carve_image(char* base, int W, int H, bool library_binning)
     return s;
 }
 
+// bits of the tile sort's keys: 2^bits > tiles, so that the pad key (all ones, emit_kernel) lies strictly above every tile index
 inline int tile_key_bits(int W, int H)
 {
     const uint32_t tiles = (uint32_t)((W + LGR_TILE - 1) / LGR_TILE) * ((H + LGR_TILE - 1) / LGR_TILE);
     int bits = 1;
-    while ((1u << bits) < tiles) bits++;
+    while ((1u << bits) <= tiles) bits++;
     return bits;
 }
 
@@ -560,11 +563,14 @@ __global__ void __launch_bounds__(256) preprocess_kernel(PreprocessArgs a, int* 
 // instances span_begin+L, +32, ... and finds each instance's owner with a 5-step shuffle binary search over the
 // warp's run offsets, so key/id stores are fully coalesced whatever the splat sizes are (the reference's one thread
 // per Gaussian loop is serial in the splat area, rasterizer_impl.cu:98-109).
+// The blob holds `capacity` instances, sized before the count R was known: instances at or past it are not written and R > capacity
+// raises HDR_OVERFLOW (the host repeats with an exact blob); slots [R, capacity) get the pad key ~0, which lies above every tile index
+// in the sort's key bits (tile_key_bits), so the pads sort last and no range reaches them.
 template <typename KeyT>
 __global__ void __launch_bounds__(256) emit_kernel(int P, const uint32_t* __restrict__ sorted_ids, const unsigned long long* __restrict__ offsets,
-                                                   const uint32_t* __restrict__ tiles_kept, const unsigned long long* __restrict__ keep_mask,
-                                                   const float2* __restrict__ means2D, const int* __restrict__ radii, int gx, int gy,
-                                                   KeyT* __restrict__ keys, uint32_t* __restrict__ ids)
+                                                   const unsigned long long* __restrict__ keep_mask, const float2* __restrict__ means2D,
+                                                   const int* __restrict__ radii, int gx, int gy, uint32_t capacity, KeyT* __restrict__ keys,
+                                                   uint32_t* __restrict__ ids, int* __restrict__ header)
 {
     const int lane = threadIdx.x & 31;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -572,10 +578,12 @@ __global__ void __launch_bounds__(256) emit_kernel(int P, const uint32_t* __rest
     int x0 = 0, y0 = 0, w = 1;
     unsigned long long mask = ~0ull;
     if (k < P) {
-        id = sorted_ids[k];
-        cnt = tiles_kept[id];
-        off = (uint32_t)offsets[k] - cnt;  // low word of the inclusive scan = kept instances up to and including k
+        // low word of the inclusive scan = kept instances up to and including k: the count comes from two adjacent (coalesced) scan
+        // words rather than a gather of tiles_kept by id, and Gaussians listed nowhere gather nothing
+        off = k > 0 ? (uint32_t)offsets[k - 1] : 0u;
+        cnt = (uint32_t)offsets[k] - off;
         if (cnt) {
+            id = sorted_ids[k];
             const float2 p = means2D[id];
             const lgr::TileRect r = lgr::tile_rect(p.x, p.y, radii[id], gx, gy);
             x0 = r.x0; y0 = r.y0; w = r.x1 - r.x0;
@@ -592,7 +600,7 @@ __global__ void __launch_bounds__(256) emit_kernel(int P, const uint32_t* __rest
     }
     if (k >= P) off = run_end;
     const uint32_t span_begin = __shfl_sync(FULL, off, 0);
-    const uint32_t span_end = __shfl_sync(FULL, run_end, 31);
+    const uint32_t span_end = min(__shfl_sync(FULL, run_end, 31), capacity);
     for (uint32_t base = span_begin; base < span_end; base += 32) {
         const uint32_t j = base + lane;
         int lo = 0, hi = 31;  // largest lane m with off[m] <= j
@@ -618,6 +626,12 @@ __global__ void __launch_bounds__(256) emit_kernel(int P, const uint32_t* __rest
             keys[j] = (KeyT)((o_y0 + ry) * gx + (o_x0 + rx));
             ids[j] = o_id;
         }
+    }
+    const uint32_t R = (uint32_t)offsets[P - 1];
+    if (R > capacity) {
+        if (k == 0) header[HDR_OVERFLOW] = 1;
+    } else {
+        for (uint32_t j = R + (uint32_t)k; j < capacity; j += gridDim.x * blockDim.x) keys[j] = (KeyT)~0u;
     }
 }
 
@@ -1081,6 +1095,15 @@ struct SyncEvent {
 };
 thread_local SyncEvent t_event;
 std::atomic<uint64_t> g_bin_overflows{0};
+std::atomic<uint64_t> g_forward_syncs{0};   // stream synchronisations of the forwards (exactly sized binning blobs)
+
+// LGR_BINNING_SYNC=1: the library binning sizes its blob exactly after a stream synchronisation, as deterministic mode does (tests
+// compare the default's estimated, padded lists against it)
+bool binning_sync_requested()
+{
+    const char* e = std::getenv("LGR_BINNING_SYNC");
+    return e && e[0] == '1';
+}
 
 __global__ void set_capacity_kernel(int* header, int capacity, int det)
 {
@@ -1132,6 +1155,38 @@ int det_tile_sort(const BinningState& bin, int R, int bits, bool debug, cudaStre
     det_point_list_kernel<<<(R + 255) / 256, 256, 0, stream>>>(R, perm, bin.ids_unsorted, bin.point_list);
     LGR_LAUNCH_CHECK("det_point_list_kernel", debug, stream);
     LGR_CUDA_TRY(cudaMemsetAsync(bin.det_reached, 0, sizeof(uint32_t) * (((size_t)R + 31) / 32), stream));
+    return LGR_OK;
+}
+
+// K2 + tile sort + K3 of the library binning over `items` instances of a blob that holds `capacity` (items == capacity, or the exact
+// count R <= capacity): emit (pads and overflow flag, see emit_kernel), stable radix sort by tile, per-tile ranges
+template <typename KeyT>
+int tile_binning(const GeometryState& geo, const BinningState& bin, const ImageState& img, const int32_t* radii, int P, int items,
+                 int capacity, int gx, int gy, int bits, bool det, bool debug, cudaStream_t stream)
+{
+    {
+        ProfScope ps(ST_EMIT, stream);
+        emit_kernel<KeyT><<<(P + 255) / 256, 256, 0, stream>>>(P, geo.sorted_ids, geo.offsets, geo.keep_mask, geo.means2D,
+                                                                 radii, gx, gy, (uint32_t)capacity, (KeyT*)bin.keys_unsorted,
+                                                                 bin.ids_unsorted, geo.num_rendered);
+    }
+    LGR_LAUNCH_CHECK("emit_kernel", debug, stream);
+    {
+        ProfScope ps(ST_TILE_SORT, stream);
+        if (det) {
+            const int st = det_tile_sort<KeyT>(bin, items, bits, debug, stream);
+            if (st != LGR_OK) return st;
+        } else {
+            size_t tmp = bin.cub_temp_bytes;
+            LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const KeyT*)bin.keys_unsorted, (KeyT*)bin.keys_sorted,
+                                                          (const uint32_t*)bin.ids_unsorted, bin.point_list, items, 0, bits, stream));
+        }
+    }
+    {
+        ProfScope ps(ST_RANGES, stream);
+        ranges_kernel<KeyT><<<(gx * gy + 255) / 256, 256, 0, stream>>>(items, gx * gy, (const KeyT*)bin.keys_sorted, img.ranges);
+    }
+    LGR_LAUNCH_CHECK("ranges_kernel", debug, stream);
     return LGR_OK;
 }
 
@@ -1380,6 +1435,7 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
         };
         if (exact) {
             LGR_CUDA_TRY(cudaStreamSynchronize(stream));
+            g_forward_syncs.fetch_add(1, std::memory_order_relaxed);
             R = host_hdr[HDR_LISTED];
             R_ref = host_hdr[HDR_RENDERED];
             int st = exact_blob();
@@ -1408,9 +1464,33 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
             g_bin_hint.store(std::max(want, keep), std::memory_order_relaxed);
         }
     } else {
-        // ---------------- round-1 path: library radix sorts and scan ----------------
+        // ---------------- library radix sorts and scan ----------------
+        // Default: the binning blob is sized from the running estimate before the count is known, and emit, tile sort, ranges and blend
+        // are queued behind the count's copy to the host, so the GPU never waits for the host (the scheme of the hand-written binning
+        // above).  Deterministic mode, and LGR_BINNING_SYNC=1, size the blob exactly after a stream synchronisation.
+        const bool exact = det || binning_sync_requested();
+        size_t capacity = 0;
+        auto carve = [&](size_t instances) -> int {   // (re)allocate the blob for `instances` and tell the device
+            bin = carve_binning(nullptr, instances, W, H, true, det);
+            char* bin_blob = binning_alloc(binning_user, bin.total);
+            if (!bin_blob) { g_last_error = "binning allocator returned NULL"; return LGR_ERR_ALLOC; }
+            bin = carve_binning(bin_blob, instances, W, H, true, det);
+            set_capacity_kernel<<<1, 32, 0, stream>>>(geo.num_rendered, instances > 0 ? (int)instances : 1, det ? 1 : 0);
+            LGR_LAUNCH_CHECK("set_capacity_kernel", debug, stream);
+            return LGR_OK;
+        };
+        const int bits = tile_key_bits(W, H);
+        auto binning = [&](int items, int cap) -> int {
+            return bin.wide_keys ? tile_binning<uint32_t>(geo, bin, img, radii, P, items, cap, gx, gy, bits, det, debug, stream)
+                                 : tile_binning<uint16_t>(geo, bin, img, radii, P, items, cap, gx, gy, bits, det, debug, stream);
+        };
         LGR_CUDA_TRY(cudaMemsetAsync(geo.num_rendered, 0, 64 * sizeof(int), stream));
         LGR_CUDA_TRY(cudaMemsetAsync(img.ranges, 0, sizeof(uint2) * (size_t)gx * gy, stream));
+        if (!exact) {
+            capacity = std::min(std::max(g_bin_hint.load(std::memory_order_relaxed), (size_t)4096), (size_t)INT_MAX);
+            const int st = carve(capacity);
+            if (st != LGR_OK) return st;
+        }
         size_t tmp = geo.cub_temp_bytes;
         {
             ProfScope ps(ST_DEPTH_SORT, stream);
@@ -1425,63 +1505,34 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
         }
         LGR_CUDA_TRY(cudaMemcpyAsync(geo.num_rendered, geo.offsets + (P - 1), 2 * sizeof(int), cudaMemcpyDeviceToDevice, stream));
         LGR_CUDA_TRY(cudaMemcpyAsync(host_hdr, geo.offsets + (P - 1), 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-        LGR_CUDA_TRY(cudaStreamSynchronize(stream));
-        R = host_hdr[0];       // instances actually emitted (after exact tile culling)
-        R_ref = host_hdr[1];   // the reference's num_rendered: sum of the tile-rectangle areas
-        bin = carve_binning(nullptr, (size_t)R, W, H, true, det);
-        char* bin_blob = binning_alloc(binning_user, bin.total);
-        if (!bin_blob) { g_last_error = "binning allocator returned NULL"; return LGR_ERR_ALLOC; }
-        bin = carve_binning(bin_blob, (size_t)R, W, H, true, det);
-        set_capacity_kernel<<<1, 32, 0, stream>>>(geo.num_rendered, R > 0 ? R : 1, det ? 1 : 0);
-        LGR_LAUNCH_CHECK("set_capacity_kernel", debug, stream);
-
-        if (R > 0) {
-            const int blocks = (P + 255) / 256;
-            const int bits = tile_key_bits(W, H);
-            tmp = bin.cub_temp_bytes;
-            if (bin.wide_keys) {
-                {
-                    ProfScope ps(ST_EMIT, stream);
-                    emit_kernel<uint32_t><<<blocks, 256, 0, stream>>>(P, geo.sorted_ids, geo.offsets, geo.tiles_kept, geo.keep_mask, geo.means2D,
-                                                                       radii, gx, gy, (uint32_t*)bin.keys_unsorted, bin.ids_unsorted);
-                }
-                LGR_LAUNCH_CHECK("emit_kernel", debug, stream);
-                {
-                    ProfScope ps(ST_TILE_SORT, stream);
-                    if (det) {
-                        const int st = det_tile_sort<uint32_t>(bin, R, bits, debug, stream);
-                        if (st != LGR_OK) return st;
-                    } else
-                        LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const uint32_t*)bin.keys_unsorted,
-                                                                      (uint32_t*)bin.keys_sorted, (const uint32_t*)bin.ids_unsorted,
-                                                                      bin.point_list, R, 0, bits, stream));
-                }
-                ProfScope ps(ST_RANGES, stream);
-                ranges_kernel<uint32_t><<<(gx * gy + 255) / 256, 256, 0, stream>>>(R, gx * gy, (const uint32_t*)bin.keys_sorted, img.ranges);
-            } else {
-                {
-                    ProfScope ps(ST_EMIT, stream);
-                    emit_kernel<uint16_t><<<blocks, 256, 0, stream>>>(P, geo.sorted_ids, geo.offsets, geo.tiles_kept, geo.keep_mask, geo.means2D,
-                                                                       radii, gx, gy, (uint16_t*)bin.keys_unsorted, bin.ids_unsorted);
-                }
-                LGR_LAUNCH_CHECK("emit_kernel", debug, stream);
-                {
-                    ProfScope ps(ST_TILE_SORT, stream);
-                    if (det) {
-                        const int st = det_tile_sort<uint16_t>(bin, R, bits, debug, stream);
-                        if (st != LGR_OK) return st;
-                    } else
-                        LGR_CUDA_TRY(cub::DeviceRadixSort::SortPairs(bin.cub_temp, tmp, (const uint16_t*)bin.keys_unsorted,
-                                                                      (uint16_t*)bin.keys_sorted, (const uint32_t*)bin.ids_unsorted,
-                                                                      bin.point_list, R, 0, bits, stream));
-                }
-                ProfScope ps(ST_RANGES, stream);
-                ranges_kernel<uint16_t><<<(gx * gy + 255) / 256, 256, 0, stream>>>(R, gx * gy, (const uint16_t*)bin.keys_sorted, img.ranges);
+        int st = LGR_OK;
+        if (exact) {
+            LGR_CUDA_TRY(cudaStreamSynchronize(stream));
+            g_forward_syncs.fetch_add(1, std::memory_order_relaxed);
+            R = host_hdr[0];       // instances actually emitted (after exact tile culling)
+            R_ref = host_hdr[1];   // the reference's num_rendered: sum of the tile-rectangle areas
+            if ((st = carve((size_t)R)) != LGR_OK) return st;
+            if (R > 0 && (st = binning(R, R)) != LGR_OK) return st;
+            if ((st = launch_blend()) != LGR_OK) return st;
+        } else {
+            // all `capacity` slots are sorted: the pads past R sort last and no range reaches them (emit_kernel)
+            cudaEvent_t ev = t_event.get();
+            LGR_CUDA_TRY(cudaEventRecord(ev, stream));
+            if ((st = binning((int)capacity, (int)capacity)) != LGR_OK) return st;
+            if ((st = launch_blend()) != LGR_OK) return st;
+            LGR_CUDA_TRY(cudaEventSynchronize(ev));
+            R = host_hdr[0];
+            R_ref = host_hdr[1];
+            if ((size_t)R > capacity) {   // estimate too small (first view, or a jump between views): the blend returned early; repeat
+                if ((st = carve((size_t)R)) != LGR_OK) return st;
+                if ((st = binning(R, R)) != LGR_OK) return st;
+                if ((st = launch_blend()) != LGR_OK) return st;
+                g_bin_overflows.fetch_add(1, std::memory_order_relaxed);
             }
-            LGR_LAUNCH_CHECK("ranges_kernel", debug, stream);
+            // next estimate: 25 % above this view, never dropping by more than 2 % per view (as the hand-written binning's)
+            const size_t want = (size_t)R + (size_t)R / 4 + 4096, keep = g_bin_hint.load(std::memory_order_relaxed) / 50 * 49;
+            g_bin_hint.store(std::max(want, keep), std::memory_order_relaxed);
         }
-        const int st = launch_blend();
-        if (st != LGR_OK) return st;
     }
     if (count_mode && P > 0) {
         ProfScope ps(ST_SCORE, stream);
@@ -1573,6 +1624,7 @@ int lgr_set_vq_mode(int mode)
 }
 
 uint64_t lgr_binning_overflows(void) { return g_bin_overflows.load(); }
+uint64_t lgr_forward_stream_syncs(void) { return g_forward_syncs.load(); }
 void lgr_set_binning_estimate(uint64_t instances) { g_bin_hint.store((size_t)instances); }
 
 int lgr_set_tile_culling(int on)
