@@ -207,6 +207,32 @@ int lgr_backward_raw_end(const lgr_view* view, int P, int M, const lgr_raw_param
 int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_params* params, const int32_t* radii, char* geometry_blob,
                                const lgr_raw_grads* grads, float* dL_dmeans2D, int first, int count, void* cuda_stream);
 
+/* ---- depth and alpha planes (DESIGN.md section 7, "Depth and alpha maps") ----
+ * For pixel p let w_i = alpha_i * T_i be the weight the colour blend gives Gaussian i, in the colour's float32 operations and order
+ * (fma(T, alpha * c, acc)), and z_i the view-space depth of the geometry blob.
+ *   depth_mode 1 ("z"):       out_depth[p] = sum_i w_i * z_i         (background 0, not divided by alpha)
+ *   depth_mode 2 ("inverse"): out_depth[p] = sum_i w_i * (1/z_i)     (1/z_i correctly rounded: torch's 1 / z in float32)
+ *   out_alpha[p] = fl(1 - final_T[p])
+ * Both planes are [H,W] float32 on the device and fully written (0 in empty tiles).
+ * lgr_forward_raw_depth: the lgr_forward_raw contract plus depth_mode (0 = none, 1 = z, 2 = inverse), out_depth and out_alpha.
+ * Either output may be NULL; out_depth needs depth_mode 1 or 2; with both NULL the call is lgr_forward_raw.  Every other output is
+ * bit-identical to lgr_forward_raw's.  Count mode, deterministic mode and the round-1 blend kernels have no depth or alpha output:
+ * LGR_ERR_INVALID_ARG, nothing launched.  The forward records its depth mode in the geometry blob.
+ * lgr_backward_raw_depth: the lgr_backward_raw contract plus the forward's depth_mode and dL_ddepth / dL_dalpha ([H,W], either may
+ * be NULL, meaning zero; with both NULL the call is lgr_backward_raw).  When the geometry blob comes from a forward that ran
+ * without depth or alpha, or in another depth_mode, every gradient of a visible Gaussian is NaN. */
+int lgr_forward_raw_depth(const lgr_view* view, int P, int M, const lgr_raw_params* params,
+                          lgr_alloc_fn geometry_alloc, void* geometry_user,
+                          lgr_alloc_fn binning_alloc, void* binning_user,
+                          lgr_alloc_fn image_alloc, void* image_user,
+                          float* out_color, int32_t* gaussians_count, float* important_score,
+                          int depth_mode, float* out_depth, float* out_alpha,
+                          int32_t* radii, int32_t* num_rendered, void* cuda_stream);
+int lgr_backward_raw_depth(const lgr_view* view, int P, int M, int num_rendered, const lgr_raw_params* params,
+                           const int32_t* radii, char* geometry_blob, char* binning_blob, char* image_blob,
+                           const float* dL_dout_color, int depth_mode, const float* dL_ddepth, const float* dL_dalpha,
+                           const lgr_raw_grads* grads, float* dL_dmeans2D, void* cuda_stream);
+
 /* View-parallel training: for one view dL/dSH[k][c] = basis_k(dir) * dRGB[c] is rank-1 per Gaussian
  * (RAST/cuda_rasterizer/backward.cu:44-97), so ranks exchange dRGB (12 B/Gaussian/view, all-gather) instead of the
  * dense 12*M B/Gaussian gradient, and each rank rebuilds the SUM over views here:

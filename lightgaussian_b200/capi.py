@@ -135,6 +135,14 @@ def load():
         lib.lgr_backward_raw.restype = i32
         lib.lgr_backward_raw.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
                                          C.POINTER(LgrRawGrads), vp, vp]
+        # depth and alpha planes: lgr_forward_raw's arguments with (depth_mode, out_depth, out_alpha) behind important_score, and
+        # lgr_backward_raw's with (depth_mode, dL_ddepth, dL_dalpha) behind dL_dout_color
+        lib.lgr_forward_raw_depth.restype = i32
+        lib.lgr_forward_raw_depth.argtypes = [C.POINTER(LgrView), i32, i32, C.POINTER(LgrRawParams), ALLOC_FN, vp, ALLOC_FN, vp, ALLOC_FN,
+                                              vp, vp, vp, vp, i32, vp, vp, vp, C.POINTER(C.c_int32), vp]
+        lib.lgr_backward_raw_depth.restype = i32
+        lib.lgr_backward_raw_depth.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
+                                               i32, vp, vp, C.POINTER(LgrRawGrads), vp, vp]
         lib.lgr_backward_raw_begin.restype = i32
         lib.lgr_backward_raw_begin.argtypes = [C.POINTER(LgrView), i32, i32, vp, vp, vp, vp, vp, vp, vp]
         lib.lgr_backward_raw_end.restype = i32
@@ -316,9 +324,18 @@ def binning_layout(R: int, W: int, H: int):
     return dict(point_list=int(out[0])), int(total)
 
 
+_blend_mode = [0]
+
+
 def set_blend_mode(mode: int) -> None:
     """0 = ring kernels (default), 1 = round-1 kernels (A/B measurements)"""
     check(load().lgr_set_blend_mode(int(mode)), "lgr_set_blend_mode")
+    _blend_mode[0] = int(mode)
+
+
+def blend_mode() -> int:
+    """the blend kernels set_blend_mode selected last in this process (0 until it is called)"""
+    return _blend_mode[0]
 
 
 DEFAULT_BINNING_MODE = 2

@@ -52,6 +52,11 @@ __device__ __forceinline__ void mbar_wait_ring(uint64_t* bar, uint32_t parity)
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// two float atomic adds to consecutive words as one vector reduction (SASS REDG.E.ADD.F32x2); `addr` must be 8-byte aligned
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b)
+{
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
 // four float atomic adds to consecutive words as ONE vector reduction (sm_90, SASS REDG.E.ADD.F32x4): one L2 operation instead of four.
 // `addr` must be 16-byte aligned.  Like atomicAdd on f32, it flushes subnormals to zero.
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d)
@@ -173,16 +178,30 @@ __device__ __forceinline__ void ring_init(BlendRing& r, int consumers)
 // being the share of the pixel's colour the Gaussian supplies (DESIGN section 3, "Blending-weight significance").  q < 0.99*2^32
 // fits 32 bits; the warp sums each 16-bit half with REDUX (< 2^21, exact) and lane 0 adds them with one 64-bit integer atomic, so the
 // per-view sums are exact and independent of every ordering.
-template <bool COUNT, bool STORE, bool PERM = false, bool WEIGHT = false>
+// DEPTH (lgr_forward_raw_depth, DESIGN section 7): the producer also stores each Gaussian's depth value (z, 1/z, or 0 when only alpha
+// is wanted) in record word 11, each lane blends it with the pixel's colour weights in the colour's operation order, and the epilogue
+// writes the depth plane sum_i alpha_i*T_i*value_i and the alpha plane fl(1 - final_T); the mode goes to header word HDR_DEPTH.
+struct BlendDepth {
+    const float* z;   // [P] view-space depth of the geometry blob
+    float* depth;     // [H,W] out, or NULL
+    float* alpha;     // [H,W] out, or NULL
+    int* header;      // the geometry header (HDR_DEPTH := 1 + mode)
+    int mode;         // 0 = alpha only (value 0), 1 = z, 2 = 1/z (correctly rounded)
+};
+
+template <bool COUNT, bool STORE, bool PERM = false, bool WEIGHT = false, bool DEPTH = false>
 __global__ void __launch_bounds__(BL_THREADS)
 blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H, int tiles_x,
                           const float2* __restrict__ means2D, const float4* __restrict__ conic_opacity, const float4* __restrict__ rgb,
                           const float* __restrict__ bg, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
                           float* __restrict__ out_color, int* __restrict__ count, float* __restrict__ rec_out, const int* __restrict__ header,
-                          const uint32_t* __restrict__ perm = nullptr, unsigned long long* __restrict__ weight = nullptr)
+                          const uint32_t* __restrict__ perm = nullptr, unsigned long long* __restrict__ weight = nullptr,
+                          BlendDepth dz = BlendDepth{})
 {
     static_assert(!WEIGHT || COUNT, "the blending weight is a count-mode output");
+    static_assert(!DEPTH || (!COUNT && STORE && !PERM && !WEIGHT), "depth and alpha are outputs of the default training forward only");
     if (header[HDR_OVERFLOW]) return;   // the binning blob was too small for this view: the host repeats scatter + blend (lgr_bin.cuh)
+    if (DEPTH && blockIdx.x == 0 && threadIdx.x == 0) dz.header[HDR_DEPTH] = 1 + dz.mode;
     __shared__ __align__(128) BlendRing ring;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x;
@@ -217,7 +236,9 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
                 float4* r4 = reinterpret_cast<float4*>(&ring.rec[s][lane * BL_REC]);
                 r4[0] = make_float4(xy.x, xy.y, co.x, co.y);
                 r4[1] = make_float4(co.z, co.w, col.x, col.y);
-                r4[2] = make_float4(col.z, __uint_as_float(id), PERM ? __uint_as_float(perm[pos0 + lane]) : 0.f, 0.f);
+                float zv = 0.f;
+                if (DEPTH && dz.mode != 0) zv = dz.mode == 2 ? __frcp_rn(dz.z[id]) : dz.z[id];
+                r4[2] = make_float4(col.z, __uint_as_float(id), PERM ? __uint_as_float(perm[pos0 + lane]) : 0.f, zv);
             }
             if (lane == 0) ring.count[s] = n;
             if (STORE) fence_async_smem();
@@ -244,6 +265,7 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
 
     float T = inside ? 1.0f : -1.0f;  // sign = "done"
     float C0 = 0.f, C1 = 0.f, C2 = 0.f;
+    float Cz = 0.f;   // DEPTH: the depth value's blend
     uint32_t last = 0;
     bool warp_done = __all_sync(FULL, T < 0.f);
     if (warp_done && lane == 0) atomicSub(&ring.live, 1);
@@ -285,6 +307,7 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
                             C0 = LGR_FMA(T, LGR_MUL(alpha, q1.z), C0);
                             C1 = LGR_FMA(T, LGR_MUL(alpha, q1.w), C1);
                             C2 = LGR_FMA(T, LGR_MUL(alpha, b), C2);
+                            if (DEPTH) Cz = LGR_FMA(T, LGR_MUL(alpha, r[11]), Cz);
                             if (WEIGHT) q = __float2uint_rn(__fmul_rn(__fmul_rn(alpha, T), 4294967296.0f));   // 2^32: exact scaling
                             T = test_T;
                             last = pos_base + (uint32_t)j;
@@ -317,6 +340,10 @@ blend_forward_ring_kernel(const uint2* __restrict__ ranges, const uint32_t* __re
         out_color[pix] = LGR_FMA(bg[0], Tf, C0);
         out_color[plane + pix] = LGR_FMA(bg[1], Tf, C1);
         out_color[2 * plane + pix] = LGR_FMA(bg[2], Tf, C2);
+        if (DEPTH) {
+            if (dz.depth) dz.depth[pix] = Cz;
+            if (dz.alpha) dz.alpha[pix] = __fsub_rn(1.0f, Tf);
+        }
     }
 }
 
@@ -327,7 +354,7 @@ struct BlendBackWarp {
     float w[BL_FLUSH][BL_ROW];     // alpha*T per (buffered pair, lane)
     float g[BL_FLUSH][BL_ROW];     // G*dL/dalpha
     float mid[BL_FLUSH], mgx[BL_FLUSH], mgy[BL_FLUSH];   // per buffered pair: Gaussian id (bits), mean2D.x, mean2D.y
-    float4 d[32];                  // the lanes' dL/dpix (r, g, b, -)
+    float4 d[32];                  // the lanes' dL/dpix (r, g, b) and, DEPTH, dL/ddepth
 };
 
 // Deterministic mode: instead of float atomics, each consumer warp parks its 9 sums of every record it blended in this block of
@@ -354,12 +381,14 @@ __host__ __device__ __forceinline__ size_t det_ids_offset(size_t Rn)   // ids_un
 
 // contract the buffered pairs of one warp and add them to the accumulator records (see the header comment).  DET: `acc` is the
 // warp's slice of BlendDetStage::c for the current stage and bw.mid holds the record's slot in the chunk; plain stores, no atomics.
-template <bool DET = false>
+// DEPTH: a tenth sum, sum_l w[l] * dL/ddepth[l] = dL/d(depth value), goes to word 9 together with word 8 (one 8-byte reduction).
+template <bool DET = false, bool DEPTH = false>
 __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, int lane, float ox, float oy, float* __restrict__ acc)
 {
     __syncwarp();
     const int p = lane & 15, h = lane >> 4;
     float c0 = 0.f, c1 = 0.f, c2 = 0.f, s0 = 0.f, mx = 0.f, my = 0.f, mxx = 0.f, mxy = 0.f, myy = 0.f;
+    float cz = 0.f;
     const float* wr = &bw.w[p][16 * h];
     const float* gr = &bw.g[p][16 * h];
     const float4* dr = &bw.d[16 * h];
@@ -371,6 +400,7 @@ __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, in
         c0 = fmaf(w, d.x, c0);
         c1 = fmaf(w, d.y, c1);
         c2 = fmaf(w, d.z, c2);
+        if (DEPTH) cz = fmaf(w, d.w, cz);
         s0 += g;
         mx = fmaf(g, xl, mx);
         my = fmaf(g, yl, my);
@@ -393,6 +423,7 @@ __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, in
     s2xx += __shfl_xor_sync(FULL, s2xx, 16);
     s2xy += __shfl_xor_sync(FULL, s2xy, 16);
     s2yy += __shfl_xor_sync(FULL, s2yy, 16);
+    if (DEPTH) cz += __shfl_xor_sync(FULL, cz, 16);
     if (DET && p < nbuf) {
         float* row = acc + __float_as_uint(bw.mid[p]) * DET_ROW;
         if (h == 0) {
@@ -407,6 +438,9 @@ __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, in
         float* rec = acc + (size_t)__float_as_uint(bw.mid[p]) * ACC_STRIDE;
         if (h == 0) {
             red_add_v4(rec, c0, c1, c2, s0);
+        } else if (DEPTH) {
+            red_add_v4(rec + 4, s1x, s1y, s2xx, s2xy);
+            red_add_v2(rec + 8, s2yy, cz);
         } else {
             red_add_v4(rec + 4, s1x, s1y, s2xx, s2xy);
             atomicAdd(rec + 8, s2yy);
@@ -423,16 +457,29 @@ constexpr size_t blend_back_smem_bytes(bool zero_rows = false, bool det = false)
            (zero_rows ? (size_t)KB_ZERO_BYTES : 0);
 }
 
+// The depth variant's per-pixel inputs (lgr_backward_raw_depth).  `tag` is the HDR_DEPTH value the forward must have left: when the
+// header holds another, the records' word 11 is not this mode's depth value, and the kernel writes NaN into words 0-9 of all P
+// accumulator records instead of reading them, so every gradient shows the mismatch.
+struct BlendDepthBack {
+    const float* dL_ddepth;   // [H,W] or NULL (zero)
+    const float* dL_dalpha;   // [H,W] or NULL (zero)
+    int tag;
+    int P;
+};
+
 // DET = false: every (warp, Gaussian) sum goes into acc[id] with float atomics (acc cleared beforehand).
 // DET = true (deterministic mode): the sums of the 8 warps are added in warp order per record and written as one partial row per
 // instance, at the instance's unsorted index (record word 10), into the binning blob; det_gather_kernel then adds each Gaussian's rows
 // in ascending unsorted-index order.  The bitmap behind the rows marks the instances that got a row.  No float atomics.
-template <bool DET = false>
+// DEPTH: the depth and alpha terms (DESIGN section 7): per pixel d.w = dL/ddepth, and D starts at T_final * (bg.dL/dpix - dL/dalpha);
+// per pair cd gains value * dL/ddepth, and the flush adds the tenth sum to record word 9.
+template <bool DET = false, bool DEPTH = false>
 __global__ void __launch_bounds__(BL_THREADS)
 blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_blob, const int* __restrict__ header, int W, int H,
                            int tiles_x, const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
-                           const float* __restrict__ dL_dpix, float* __restrict__ acc, KbackZeroArgs zero)
+                           const float* __restrict__ dL_dpix, float* __restrict__ acc, KbackZeroArgs zero, BlendDepthBack db = BlendDepthBack{})
 {
+    static_assert(!(DET && DEPTH), "deterministic mode has no depth variant");
     extern __shared__ __align__(128) unsigned char blend_dyn_smem[];
     BlendRing& ring = *reinterpret_cast<BlendRing*>(blend_dyn_smem);
     BlendBackWarp* warps = reinterpret_cast<BlendBackWarp*>(blend_dyn_smem + ((sizeof(BlendRing) + 127) / 128) * 128);
@@ -463,6 +510,18 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
     if (lane == 0 && warp_max) atomicMax(&ring.tile_max, warp_max);
     __syncthreads();
     const uint32_t tile_max = ring.tile_max;
+    // DEPTH: a forward that ran without depth or in another mode left no (or another) value in record word 11: the records are not read,
+    // and NaN accumulators make the misuse show in every gradient (see BlendDepthBack)
+    if (DEPTH && header[HDR_DEPTH] != db.tag) {
+        const float nan = __int_as_float(0x7fc00000);
+        for (int i = blockIdx.x * BL_THREADS + threadIdx.x; i < db.P; i += gridDim.x * BL_THREADS) {
+            float4* rec = reinterpret_cast<float4*>(acc + (size_t)i * ACC_STRIDE);
+            rec[0] = rec[1] = make_float4(nan, nan, nan, nan);
+            rec[2] = make_float4(nan, nan, 0.f, 0.f);
+        }
+        if (zero_rows && threadIdx.x == 8 * 32) bulk_wait_all();   // the zero page must outlive the stores that read it
+        return;
+    }
     // DET: a forward that did not run in deterministic mode stored no permutation; nothing is read or written (det_gather_kernel then
     // writes NaN accumulators, so the misuse shows in every gradient instead of corrupting memory)
     if (tile_max == 0 || (DET && header[HDR_DET] != 1)) {
@@ -554,11 +613,17 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
         d1 = dL_dpix[plane + pix];
         d2 = dL_dpix[2 * plane + pix];
     }
-    bw.d[lane] = make_float4(d0, d1, d2, 0.f);
+    float dz = 0.f, da = 0.f;   // DEPTH: this pixel's dL/ddepth and dL/dalpha
+    if (DEPTH && inside) {
+        if (db.dL_ddepth) dz = db.dL_ddepth[pix];
+        if (db.dL_dalpha) da = db.dL_dalpha[pix];
+    }
+    bw.d[lane] = make_float4(d0, d1, d2, dz);
     // D = sum_c dL/dpix_c * (background + everything blended BEHIND the current Gaussian), in absolute (not T-normalised) units:
     // the reference's  T*(c - accum_rec).dpix - T_final/(1-alpha)*bg.dpix  (backward.cu:505-518) equals  T*(c.dpix) - D/(1-alpha),
     // and D grows by alpha*T*(c.dpix) per blended Gaussian -- one scalar recurrence instead of three colour recurrences.
-    float D = T_final * (bg[0] * d0 + bg[1] * d1 + bg[2] * d2);
+    // DEPTH: alpha = 1 - prod(1 - alpha_i) has dA/dalpha_i = T_final/(1 - alpha_i), the form of the background term: -dL/dalpha joins it
+    float D = DEPTH ? T_final * ((bg[0] * d0 + bg[1] * d1 + bg[2] * d2) - da) : T_final * (bg[0] * d0 + bg[1] * d1 + bg[2] * d2);
     int nbuf = 0;
     __syncwarp();
 
@@ -601,7 +666,8 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
                 asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(one_m_a));
                 rcp = fmaf(rcp, fmaf(-one_m_a, rcp, 1.0f), rcp);
                 T = T * rcp;
-                const float cd = fmaf(q1.z, d0, fmaf(q1.w, d1, q2.x * d2));
+                float cd = fmaf(q1.z, d0, fmaf(q1.w, d1, q2.x * d2));
+                if (DEPTH) cd = fmaf(r[11], dz, cd);
                 const float dL_dalpha = fmaf(T, cd, -rcp * D);
                 const float w = alpha * T;
                 D = fmaf(w, cd, D);
@@ -614,7 +680,7 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
                 }
                 if (DET) wrote |= 1u << j;
                 if (++nbuf == BL_FLUSH) {
-                    back_flush<DET>(bw, nbuf, lane, rx0, ry0, parked);
+                    back_flush<DET, DEPTH>(bw, nbuf, lane, rx0, ry0, parked);
                     nbuf = 0;
                 }
             }
@@ -628,7 +694,7 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
         __syncwarp();
         if (lane == 0) mbar_arrive(&ring.empty[s]);
     }
-    if (!DET && nbuf) back_flush(bw, nbuf, lane, rx0, ry0, acc);
+    if (!DET && nbuf) back_flush<false, DEPTH>(bw, nbuf, lane, rx0, ry0, acc);
 }
 
 // ---- deterministic mode, across tiles: the Gaussian of depth rank k owns the unsorted instances [offsets[k-1], offsets[k]) (emit

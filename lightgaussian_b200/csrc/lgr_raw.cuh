@@ -327,7 +327,27 @@ struct RawBackArgs {
     float* d_rgb;  // optional [P,3]: clamp-masked dL/dRGB (compact SH gradient factor); when set and d_rest == NULL the dense SH rows are not written
 };
 
-__global__ void __launch_bounds__(256) preprocess_backward_raw_kernel(RawBackArgs a)
+// The depth variant's extra K7+K8 input (lgr_backward_raw_depth): accumulator word 9 holds dL/d(depth value), the value being z
+// (mode 1) or the forward's correctly rounded 1/z (mode 2); dL/dz reaches dL/dxyz through z = view[2] x + view[6] y + view[10] z + view[14].
+struct RawDepth {
+    const float* z;   // [P] view-space depth of the geometry blob
+    int mode;         // 0 = alpha only (word 9 is zero), 1 = z, 2 = inverse
+};
+
+__device__ __forceinline__ void depth_grad_to_mean(const RawDepth& dz, const float* __restrict__ rec, size_t i, const float* view, float* dmean)
+{
+    float g = rec[9];
+    if (dz.mode == 2) {
+        const float r = __frcp_rn(dz.z[i]);
+        g = -(g * r) * r;
+    }
+    dmean[0] = fmaf(g, view[2], dmean[0]);
+    dmean[1] = fmaf(g, view[6], dmean[1]);
+    dmean[2] = fmaf(g, view[10], dmean[2]);
+}
+
+template <bool DEPTH>
+__device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& a, const RawDepth& dz)
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
     const int nrest = (a.M - 1) * 3;
@@ -363,6 +383,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_raw_kernel(RawBackArg
         const float4 r0 = r4[0], r1 = r4[1];
         const float r2 = a.acc[si * ACC_STRIDE + 8];
         vis = r0.x != 0.f || r0.y != 0.f || r0.z != 0.f || r0.w != 0.f || r1.x != 0.f || r1.y != 0.f || r1.z != 0.f || r1.w != 0.f || r2 != 0.f;
+        if (DEPTH) vis = vis || a.acc[si * ACC_STRIDE + 9] != 0.f;
     }
     const unsigned live = __ballot_sync(FULL, vis);
     const bool any_vis = live != 0;
@@ -387,6 +408,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_raw_kernel(RawBackArg
         for (int k = 0; k < 6; k++) c3[k] = a.cov3D[6 * si + k];
         lgr::cov2d_backward(x, y, z, view, c3, a.fx, a.fy, a.tanx, a.tany, g2.dcx, g2.dcy, g2.dcw, dcov, dmean);
         lgr::mean2d_backward(x, y, z, proj, g2.dm2x, g2.dm2y, dmean);
+        if (DEPTH) depth_grad_to_mean(dz, a.acc + si * ACC_STRIDE, si, view, dmean);
         g2x = g2.dm2x; g2y = g2.dm2y;
         const unsigned cb = a.clamped[i];
         dRGB[0] = (cb & 1u) ? 0.f : g2.dcol[0]; dRGB[1] = (cb & 2u) ? 0.f : g2.dcol[1]; dRGB[2] = (cb & 4u) ? 0.f : g2.dcol[2];
@@ -466,6 +488,9 @@ __global__ void __launch_bounds__(256) preprocess_backward_raw_kernel(RawBackArg
         for (int k = lane; k < n * 3; k += 32) a.d_dc[(size_t)first * 3 + k] = s_dc[k];
     }
 }
+
+__global__ void __launch_bounds__(256) preprocess_backward_raw_kernel(RawBackArgs a) { preprocess_backward_raw_body<false>(a, RawDepth{}); }
+__global__ void __launch_bounds__(256) preprocess_backward_raw_depth_kernel(RawBackArgs a, RawDepth dz) { preprocess_backward_raw_body<true>(a, dz); }
 
 // ------------------------------------------------------------------------------------------------------------------
 // View-parallel SH gradient.  For one view dL/dSH[k][c] = basis_k(dir) * dRGB[c] is rank-1 per Gaussian

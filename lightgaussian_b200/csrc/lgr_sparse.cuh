@@ -410,8 +410,9 @@ __global__ void __launch_bounds__(256) densify_stats_exchanged_kernel(DensifyExc
 //                             SH rows staged through shared memory row by row, results written over the zeros.  Grid-stride over
 //                             the device-side count: no host synchronisation.
 // ------------------------------------------------------------------------------------------------------------------
-template <bool ZERO>
-__global__ void __launch_bounds__(256) kback_zero_flag_kernel(KbackZeroArgs a)
+// DEPTH: word 9 (dL/d(depth value)) counts too, so a Gaussian whose only gradient comes from the depth plane is listed
+template <bool ZERO, bool DEPTH>
+__device__ __forceinline__ void kback_zero_flag_body(const KbackZeroArgs& a)
 {
     __shared__ __align__(128) float zero_page[ZERO ? KB_ZERO_BYTES / 4 : 4];
     if (ZERO) {
@@ -449,6 +450,7 @@ __global__ void __launch_bounds__(256) kback_zero_flag_kernel(KbackZeroArgs a)
         const float4 u = r[0], w = r[1];
         const float c = a.acc[(size_t)i * ACC_STRIDE + 8];
         nz = u.x != 0.f || u.y != 0.f || u.z != 0.f || u.w != 0.f || w.x != 0.f || w.y != 0.f || w.z != 0.f || w.w != 0.f || c != 0.f;
+        if (DEPTH) nz = nz || a.acc[(size_t)i * ACC_STRIDE + 9] != 0.f;
     }
     const unsigned word = __ballot_sync(FULL, nz);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -468,10 +470,17 @@ __global__ void __launch_bounds__(256) kback_zero_flag_kernel(KbackZeroArgs a)
     if (ZERO && threadIdx.x == 0 && n == 256) bulk_wait_read_all();   // the zero page must outlive the copies that read it
 }
 
+template <bool ZERO>
+__global__ void __launch_bounds__(256) kback_zero_flag_kernel(KbackZeroArgs a) { kback_zero_flag_body<ZERO, false>(a); }
+template <bool ZERO>
+__global__ void __launch_bounds__(256) kback_zero_flag_depth_kernel(KbackZeroArgs a) { kback_zero_flag_body<ZERO, true>(a); }
+
 constexpr int KC_THREADS = 128;   // compacted K7+K8: 4 warps per block
 constexpr int KC_ROW = 49;        // floats per staged SH row (48 + 1: conflict-free at one row per lane)
 
-__global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_kernel(RawBackArgs a, const int* __restrict__ idx, const int* __restrict__ counter)
+template <bool DEPTH>
+__device__ __forceinline__ void preprocess_backward_compact_body(const RawBackArgs& a, const int* __restrict__ idx, const int* __restrict__ counter,
+                                                                 const RawDepth& dz)
 {
     // SH rows (48 floats per Gaussian) are scattered in memory: each warp moves its 32 rows through shared memory with row-contiguous
     // accesses (2 + 1 instructions per row) instead of 48 strided ones per lane -- 8x fewer sectors touched for the loads and the stores
@@ -532,6 +541,7 @@ __global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_kernel
             for (int k = 0; k < 6; k++) c3[k] = a.cov3D[6 * si + k];
             lgr::cov2d_backward(x, y, z, view, c3, a.fx, a.fy, a.tanx, a.tany, g2.dcx, g2.dcy, g2.dcw, dcov, dmean);
             lgr::mean2d_backward(x, y, z, proj, g2.dm2x, g2.dm2y, dmean);
+            if (DEPTH) depth_grad_to_mean(dz, a.acc + si * ACC_STRIDE, si, view, dmean);
             const unsigned cb = a.clamped[i];
             dRGB[0] = (cb & 1u) ? 0.f : g2.dcol[0]; dRGB[1] = (cb & 2u) ? 0.f : g2.dcol[1]; dRGB[2] = (cb & 4u) ? 0.f : g2.dcol[2];
             const float s0 = act_exp(a.scaling[3 * si]), s1 = act_exp(a.scaling[3 * si + 1]), s2 = act_exp(a.scaling[3 * si + 2]);
@@ -575,6 +585,16 @@ __global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_kernel
         }
         __syncwarp();
     }
+}
+
+__global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_kernel(RawBackArgs a, const int* __restrict__ idx, const int* __restrict__ counter)
+{
+    preprocess_backward_compact_body<false>(a, idx, counter, RawDepth{});
+}
+__global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_depth_kernel(RawBackArgs a, const int* __restrict__ idx,
+                                                                                        const int* __restrict__ counter, RawDepth dz)
+{
+    preprocess_backward_compact_body<true>(a, idx, counter, dz);
 }
 
 }  // namespace

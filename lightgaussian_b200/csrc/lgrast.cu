@@ -1210,7 +1210,7 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
                  lgr_alloc_fn geometry_alloc, void* geometry_user, lgr_alloc_fn binning_alloc, void* binning_user,
                  lgr_alloc_fn image_alloc, void* image_user, float* out_color, int32_t* gaussians_count, float* important_score,
                  int32_t* radii, int32_t* num_rendered, void* cuda_stream, bool count_mode, const lgr_raw_params* raw = nullptr,
-                 const lgr_vq_resident_params* vq = nullptr, int64_t* blend_weight = nullptr)
+                 const lgr_vq_resident_params* vq = nullptr, int64_t* blend_weight = nullptr, const BlendDepth* depth_out = nullptr)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     if (vq) {  // resident VQ model: attributes and colour rows come from the compressed arrays (validated by lgr_forward_vq)
@@ -1267,6 +1267,12 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
                                          : "lgr_forward_*_weight: the blending weight is a count-mode output";
         return LGR_ERR_INVALID_ARG;
     }
+    if (depth_out && (count_mode || g_det || g_blend_mode != 0)) {
+        g_last_error = count_mode ? "lgr_forward_raw_depth: depth and alpha are not count-mode outputs"
+                       : g_det    ? "lgr_forward_raw_depth: deterministic mode has no depth or alpha output"
+                                  : "lgr_forward_raw_depth: depth and alpha need the ring blend kernels; lgr_set_blend_mode(1) has no depth output";
+        return LGR_ERR_INVALID_ARG;
+    }
     const bool debug = v->debug != 0;
     *num_rendered = 0;
     const int gx = (W + LGR_TILE - 1) / LGR_TILE, gy = (H + LGR_TILE - 1) / LGR_TILE;
@@ -1274,6 +1280,8 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
 
     if (P == 0) {  // the reference returns an all-zero image and empty blobs (rasterize_points.cu:79-93)
         LGR_CUDA_TRY(cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * N, stream));
+        if (depth_out && depth_out->depth) LGR_CUDA_TRY(cudaMemsetAsync(depth_out->depth, 0, sizeof(float) * N, stream));
+        if (depth_out && depth_out->alpha) LGR_CUDA_TRY(cudaMemsetAsync(depth_out->alpha, 0, sizeof(float) * N, stream));
         return LGR_OK;
     }
     if (((uintptr_t)rotations & 15) || ((uintptr_t)shs & 15)) {
@@ -1338,7 +1346,14 @@ int forward_impl(const lgr_view* v, int P, int M, const float* means3D, const fl
         if (count_mode) LGR_CUDA_TRY(cudaMemsetAsync(gaussians_count, 0, sizeof(int) * (size_t)P, stream));
         if (blend_weight) LGR_CUDA_TRY(cudaMemsetAsync(blend_weight, 0, sizeof(int64_t) * (size_t)P, stream));
         ProfScope ps(count_mode ? ST_BLEND_FWD_COUNT : ST_BLEND_FWD, stream);
-        if (blend_weight)   // refused above unless g_blend_mode == 0 and count_mode
+        if (depth_out) {   // refused above unless g_blend_mode == 0, not count mode and not deterministic
+            BlendDepth dz = *depth_out;
+            dz.z = geo.depth;
+            dz.header = geo.num_rendered;
+            blend_forward_ring_kernel<false, true, false, false, true><<<tiles, BL_THREADS, 0, stream>>>(
+                img.ranges, bin.point_list, W, H, gx, geo.means2D, geo.conic_opacity, geo.rgb, v->background, img.final_T, img.n_contrib,
+                out_color, nullptr, bin.records, geo.num_rendered, nullptr, nullptr, dz);
+        } else if (blend_weight)   // refused above unless g_blend_mode == 0 and count_mode
             blend_forward_ring_kernel<true, false, false, true><<<tiles, BL_THREADS, 0, stream>>>(
                 img.ranges, bin.point_list, W, H, gx, geo.means2D, geo.conic_opacity, geo.rgb, v->background, img.final_T, img.n_contrib,
                 out_color, gaussians_count, nullptr, geo.num_rendered, nullptr, reinterpret_cast<unsigned long long*>(blend_weight));
@@ -1896,9 +1911,10 @@ int lgr_forward_vq_weight(const lgr_view* view, int P, const lgr_vq_resident_par
 thread_local KbackZeroArgs t_zero_req = {};
 thread_local bool t_rows_zeroed = false;
 
-// stage 1 of the raw backward: clear the accumulators, blend backward, optionally extract this view's dL/dRGB
-int lgr_backward_raw_begin(const lgr_view* v, int P, int num_rendered, const int32_t* radii, char* geometry_blob, char* binning_blob,
-                           char* image_blob, const float* dL_dout_color, float* d_rgb, void* cuda_stream)
+// stage 1 of the raw backward: clear the accumulators, blend backward, optionally extract this view's dL/dRGB.  db: the depth variant
+// of the blend backward (lgr_backward_raw_depth; the caller refused deterministic mode and blend mode 1)
+static int backward_raw_begin_impl(const lgr_view* v, int P, int num_rendered, const int32_t* radii, char* geometry_blob, char* binning_blob,
+                                   char* image_blob, const float* dL_dout_color, float* d_rgb, void* cuda_stream, const BlendDepthBack* db)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     if (P == 0) return LGR_OK;
@@ -1932,10 +1948,18 @@ int lgr_backward_raw_begin(const lgr_view* v, int P, int num_rendered, const int
             const KbackZeroArgs zr = t_zero_req;
             t_zero_req.P = 0;
             const size_t bsmem = blend_back_smem_bytes(zr.P > 0);
-            LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes(true)));
-            blend_backward_ring_kernel<false><<<gx * gy, BL_THREADS, bsmem, stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
-                                                                                 v->background, img.final_T, img.n_contrib,
-                                                                                 dL_dout_color, geo.grad_acc, zr);
+            if (db) {
+                LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  (int)blend_back_smem_bytes(true)));
+                blend_backward_ring_kernel<false, true><<<gx * gy, BL_THREADS, bsmem, stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
+                                                                                             v->background, img.final_T, img.n_contrib,
+                                                                                             dL_dout_color, geo.grad_acc, zr, *db);
+            } else {
+                LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blend_back_smem_bytes(true)));
+                blend_backward_ring_kernel<false><<<gx * gy, BL_THREADS, bsmem, stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
+                                                                                     v->background, img.final_T, img.n_contrib,
+                                                                                     dL_dout_color, geo.grad_acc, zr);
+            }
             t_rows_zeroed = zr.P > 0;
         } else
             blend_backward_kernel<<<gx * gy, 256, 0, stream>>>(img.ranges, bin.point_list, W, H, gx, geo.means2D, geo.conic_opacity, geo.rgb,
@@ -1949,6 +1973,12 @@ int lgr_backward_raw_begin(const lgr_view* v, int P, int num_rendered, const int
     return LGR_OK;
 }
 
+int lgr_backward_raw_begin(const lgr_view* v, int P, int num_rendered, const int32_t* radii, char* geometry_blob, char* binning_blob,
+                           char* image_blob, const float* dL_dout_color, float* d_rgb, void* cuda_stream)
+{
+    return backward_raw_begin_impl(v, P, num_rendered, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, d_rgb, cuda_stream, nullptr);
+}
+
 // stage 2: the per-Gaussian backward (K7+K8 with the activation chain rules) from the accumulators left by stage 1
 int lgr_backward_raw_end(const lgr_view* v, int P, int M, const lgr_raw_params* params, const int32_t* radii, char* geometry_blob,
                          const lgr_raw_grads* grads, float* dL_dmeans2D, void* cuda_stream)
@@ -1957,9 +1987,9 @@ int lgr_backward_raw_end(const lgr_view* v, int P, int M, const lgr_raw_params* 
 }
 
 // the same for Gaussians [first, first+count) only; first must be a multiple of 256.  Lets the caller start exchanging the gradients
-// of one range while the next range is still being computed.
-int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_params* params, const int32_t* radii, char* geometry_blob,
-                               const lgr_raw_grads* grads, float* dL_dmeans2D, int first, int count, void* cuda_stream)
+// of one range while the next range is still being computed.  rd: the depth variant of K7+K8 (lgr_backward_raw_depth, whole view)
+static int backward_raw_end_impl(const lgr_view* v, int P, int M, const lgr_raw_params* params, const int32_t* radii, char* geometry_blob,
+                                 const lgr_raw_grads* grads, float* dL_dmeans2D, int first, int count, void* cuda_stream, const RawDepth* rd)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     if (P == 0 || count == 0) return LGR_OK;
@@ -2015,18 +2045,27 @@ int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_pa
         z.d_xyz = a.d_xyz; z.d_dc = a.d_dc; z.d_rest = a.d_rest; z.d_scaling = a.d_scaling; z.d_rotation = a.d_rotation; z.d_opacity = a.d_opacity;
         z.dL_dmeans2D = dL_dmeans2D;
         if (M == 1) z.d_rest = a.d_dc;   // no rest coefficients: nrest = 0, pointer unused
-        if (rows_zeroed) kback_zero_flag_kernel<false><<<(P + 255) / 256, 256, 0, stream>>>(z);
+        if (rd && rows_zeroed) kback_zero_flag_depth_kernel<false><<<(P + 255) / 256, 256, 0, stream>>>(z);
+        else if (rd) kback_zero_flag_depth_kernel<true><<<(P + 255) / 256, 256, 0, stream>>>(z);
+        else if (rows_zeroed) kback_zero_flag_kernel<false><<<(P + 255) / 256, 256, 0, stream>>>(z);
         else kback_zero_flag_kernel<true><<<(P + 255) / 256, 256, 0, stream>>>(z);
         LGR_LAUNCH_CHECK("kback_zero_flag_kernel", debug, stream);
         a.P = P;
         const int blocks = std::min((P + KC_THREADS - 1) / KC_THREADS, LGR_SMS * 8);
-        preprocess_backward_compact_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter);
+        if (rd)
+            preprocess_backward_compact_depth_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter, *rd);
+        else
+            preprocess_backward_compact_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter);
         LGR_LAUNCH_CHECK("preprocess_backward_compact_kernel", debug, stream);
         return LGR_OK;
     }
     const size_t smem = raw_smem_bytes(M);
-    LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_backward_raw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    {
+    if (rd) {
+        LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_backward_raw_depth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ProfScope ps(ST_PREPROCESS_BWD, stream);
+        preprocess_backward_raw_depth_kernel<<<(count + 255) / 256, 256, smem, stream>>>(a, *rd);
+    } else {
+        LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_backward_raw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ProfScope ps(ST_PREPROCESS_BWD, stream);
         preprocess_backward_raw_kernel<<<(count + 255) / 256, 256, smem, stream>>>(a);
     }
@@ -2034,9 +2073,15 @@ int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_pa
     return LGR_OK;
 }
 
-int lgr_backward_raw(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
-                     char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, const lgr_raw_grads* grads,
-                     float* dL_dmeans2D, void* cuda_stream)
+int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_params* params, const int32_t* radii, char* geometry_blob,
+                               const lgr_raw_grads* grads, float* dL_dmeans2D, int first, int count, void* cuda_stream)
+{
+    return backward_raw_end_impl(v, P, M, params, radii, geometry_blob, grads, dL_dmeans2D, first, count, cuda_stream, nullptr);
+}
+
+static int backward_raw_impl(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
+                             char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, const lgr_raw_grads* grads,
+                             float* dL_dmeans2D, void* cuda_stream, const BlendDepthBack* db, const RawDepth* rd)
 {
     t_zero_req.P = 0;
     t_rows_zeroed = false;
@@ -2050,10 +2095,81 @@ int lgr_backward_raw(const lgr_view* v, int P, int M, int num_rendered, const lg
         z.d_xyz = grads->xyz; z.d_dc = grads->features_dc; z.d_rest = grads->features_rest; z.d_scaling = grads->scaling;
         z.d_rotation = grads->rotation; z.d_opacity = grads->opacity; z.dL_dmeans2D = dL_dmeans2D;
     }
-    const int st = lgr_backward_raw_begin(v, P, num_rendered, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, nullptr, cuda_stream);
+    const int st = backward_raw_begin_impl(v, P, num_rendered, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, nullptr, cuda_stream, db);
     t_zero_req.P = 0;
     if (st != LGR_OK) { t_rows_zeroed = false; return st; }
-    return lgr_backward_raw_end(v, P, M, params, radii, geometry_blob, grads, dL_dmeans2D, cuda_stream);
+    return backward_raw_end_impl(v, P, M, params, radii, geometry_blob, grads, dL_dmeans2D, 0, P, cuda_stream, rd);
+}
+
+int lgr_backward_raw(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
+                     char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, const lgr_raw_grads* grads,
+                     float* dL_dmeans2D, void* cuda_stream)
+{
+    return backward_raw_impl(v, P, M, num_rendered, params, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dmeans2D,
+                             cuda_stream, nullptr, nullptr);
+}
+
+// ---- depth and alpha planes (DESIGN section 7) ----
+static bool depth_request_ok(const char* what, int depth_mode, bool depth_plane)
+{
+    if (depth_mode < 0 || depth_mode > 2) {
+        g_last_error = std::string(what) + ": depth_mode must be 0 (none), 1 (z) or 2 (inverse)";
+        return false;
+    }
+    if (depth_plane && depth_mode == 0) {
+        g_last_error = std::string(what) + ": a depth plane needs depth_mode 1 (z) or 2 (inverse)";
+        return false;
+    }
+    if (g_det) {
+        g_last_error = std::string(what) + ": deterministic mode has no depth or alpha output";
+        return false;
+    }
+    if (g_blend_mode != 0) {
+        g_last_error = std::string(what) + ": depth and alpha need the ring blend kernels; lgr_set_blend_mode(1) has no depth output";
+        return false;
+    }
+    return true;
+}
+
+int lgr_forward_raw_depth(const lgr_view* view, int P, int M, const lgr_raw_params* params, lgr_alloc_fn geometry_alloc, void* geometry_user,
+                          lgr_alloc_fn binning_alloc, void* binning_user, lgr_alloc_fn image_alloc, void* image_user, float* out_color,
+                          int32_t* gaussians_count, float* important_score, int depth_mode, float* out_depth, float* out_alpha,
+                          int32_t* radii, int32_t* num_rendered, void* cuda_stream)
+{
+    if (!out_depth && !out_alpha)
+        return lgr_forward_raw(view, P, M, params, geometry_alloc, geometry_user, binning_alloc, binning_user, image_alloc, image_user,
+                               out_color, gaussians_count, important_score, radii, num_rendered, cuda_stream);
+    if (!depth_request_ok("lgr_forward_raw_depth", depth_mode, out_depth != nullptr)) return LGR_ERR_INVALID_ARG;
+    if (!params || M < 1) {
+        g_last_error = "lgr_forward_raw_depth: params missing or M < 1";
+        return LGR_ERR_INVALID_ARG;
+    }
+    BlendDepth dz = {};
+    dz.depth = out_depth;
+    dz.alpha = out_alpha;
+    dz.mode = depth_mode;
+    return forward_impl(view, P, M, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, geometry_alloc, geometry_user,
+                        binning_alloc, binning_user, image_alloc, image_user, out_color, gaussians_count, important_score, radii,
+                        num_rendered, cuda_stream, gaussians_count != nullptr, params, nullptr, nullptr, &dz);
+}
+
+int lgr_backward_raw_depth(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
+                           char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, int depth_mode,
+                           const float* dL_ddepth, const float* dL_dalpha, const lgr_raw_grads* grads, float* dL_dmeans2D, void* cuda_stream)
+{
+    if (!dL_ddepth && !dL_dalpha)
+        return lgr_backward_raw(v, P, M, num_rendered, params, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, grads,
+                                dL_dmeans2D, cuda_stream);
+    if (!depth_request_ok("lgr_backward_raw_depth", depth_mode, dL_ddepth != nullptr)) return LGR_ERR_INVALID_ARG;
+    if (P == 0) return LGR_OK;
+    if (!geometry_blob) {
+        g_last_error = "lgr_backward_raw_depth: missing required argument";
+        return LGR_ERR_INVALID_ARG;
+    }
+    const BlendDepthBack db = {dL_ddepth, dL_dalpha, 1 + depth_mode, P};
+    const RawDepth rd = {carve_geometry(geometry_blob, (size_t)P, false).depth, depth_mode};
+    return backward_raw_impl(v, P, M, num_rendered, params, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dmeans2D,
+                             cuda_stream, &db, &rd);
 }
 
 // ---- sparse view-parallel exchange (lgr_sparse.cuh) ----

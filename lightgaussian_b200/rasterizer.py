@@ -21,7 +21,7 @@ import os as _os
 import torch
 import torch.nn as nn
 
-from . import capi
+from . import capi, trace
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -337,8 +337,9 @@ def _raw_struct(xyz, dc, rest, scaling, rotation, opacity):
                              0 if dense else rest_row_stride(rest))
 
 
-def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacity, blend_weight=None):
-    """blend_weight: optional int64 [P] output of a count forward (lgr_forward_raw_weight), as in _forward_native."""
+def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacity, blend_weight=None, depth=None):
+    """blend_weight: optional int64 [P] output of a count forward (lgr_forward_raw_weight), as in _forward_native.
+    depth: optional (depth_mode, out_depth, out_alpha) of lgr_forward_raw_depth, the two planes [H,W]-sized float32 tensors or None."""
     lib = capi.load()
     device = xyz.device
     P, H, W = xyz.size(0), int(rs.image_height), int(rs.image_width)
@@ -370,9 +371,11 @@ def _forward_raw_native(count_mode, rs, xyz, dc, rest, scaling, rotation, opacit
             tail = (capi.ptr(radii), C.byref(num_rendered), capi.current_stream_ptr(device))
             if weight is not None:
                 st = lib.lgr_forward_raw_weight(*head, capi.ptr(weight), *tail)
+            elif depth is not None:
+                st = lib.lgr_forward_raw_depth(*head, int(depth[0]), capi.ptr(depth[1]), capi.ptr(depth[2]), *tail)
             else:
                 st = lib.lgr_forward_raw(*head, *tail)
-        capi.check(st, "lgr_forward_raw_weight" if weight is not None else "lgr_forward_raw")
+        capi.check(st, "lgr_forward_raw_weight" if weight is not None else "lgr_forward_raw_depth" if depth is not None else "lgr_forward_raw")
     finally:
         for s_ in slots:
             s_.release()
@@ -515,6 +518,111 @@ class _RasterizeRawLeaves(torch.autograd.Function):
             g, g2d = _backward_raw_exchange(rs, ctx.num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom,
                                             binning, img, world, _exchange["group"])
         return g[0], g2d, g[1], g[2], g[3], g[4], g[5], None
+
+
+DEPTH_MODES = {"z": 1, "inverse": 2}
+
+
+def depth_alpha_refusal() -> str | None:
+    """Why the fused node cannot return depth / alpha under the current settings, or None.  Checked before any launch."""
+    if capi.deterministic_requested():
+        return "deterministic mode (LGR_DETERMINISTIC=1 or torch.use_deterministic_algorithms) has no depth or alpha output"
+    if capi.blend_mode() != 0:
+        return "blend mode 1 (the round-1 blend kernels) has no depth or alpha output"
+    if _exchange["world"] > 1:
+        return "the view-parallel gradient exchange has no depth or alpha backward"
+    if _os.environ.get("LGR_SPARSE_SINGLE", "0") == "1":
+        return "LGR_SPARSE_SINGLE=1 (the sparse single-GPU backward) has no depth or alpha backward"
+    return None
+
+
+class _RasterizeRawLeavesDepth(torch.autograd.Function):
+    """render(depth=..., alpha=...)'s node: _RasterizeRawLeaves plus the depth and alpha planes ([1,H,W] each; an empty placeholder
+    for one that was not asked for).  The backward takes the existing lgr_backward_raw when neither plane received a gradient."""
+
+    @staticmethod
+    def forward(ctx, xyz, means2D, dc, rest, scaling, rotation, opacity, raster_settings, depth_mode, want_depth, want_alpha):
+        H, W = int(raster_settings.image_height), int(raster_settings.image_width)
+        plane = lambda on: torch.empty((1, H, W), dtype=torch.float32, device=xyz.device) if on else None  # noqa: E731
+        out_depth, out_alpha = plane(want_depth), plane(want_alpha)
+        _, _, R, color, radii, geom, binning, img, leaves = _forward_raw_native(False, raster_settings, xyz, dc, rest, scaling, rotation,
+                                                                                opacity, depth=(depth_mode, out_depth, out_alpha))
+        ctx.raster_settings = raster_settings
+        ctx.num_rendered = R
+        ctx.depth_mode = depth_mode
+        ctx.save_for_backward(*leaves, radii, geom, binning, img)
+        ctx.set_materialize_grads(False)
+        empty = lambda: torch.empty((0,), dtype=torch.float32, device=xyz.device)  # noqa: E731
+        out_depth = out_depth if out_depth is not None else empty()
+        out_alpha = out_alpha if out_alpha is not None else empty()
+        ctx.mark_non_differentiable(radii)
+        if not want_depth:
+            ctx.mark_non_differentiable(out_depth)
+        if not want_alpha:
+            ctx.mark_non_differentiable(out_alpha)
+        return color, radii, out_depth, out_alpha
+
+    @staticmethod
+    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha):
+        rs = ctx.raster_settings
+        xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img = ctx.saved_tensors
+        H, W = int(rs.image_height), int(rs.image_width)
+        if grad_out_color is None:
+            grad_out_color = torch.zeros((3, H, W), dtype=torch.float32, device=xyz.device)
+        if grad_depth is not None and grad_depth.numel() == 0:
+            grad_depth = None
+        if grad_alpha is not None and grad_alpha.numel() == 0:
+            grad_alpha = None
+        if grad_depth is None and grad_alpha is None:
+            trace.bump("raw_backward_plain")
+            g, g2d, _, _ = backward_raw_native(rs, ctx.num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii,
+                                               geom, binning, img, compact=False)
+        else:
+            trace.bump("raw_backward_depth")
+            g, g2d = backward_raw_depth_native(rs, ctx.num_rendered, grad_out_color, ctx.depth_mode, grad_depth, grad_alpha, xyz, dc,
+                                               rest, scaling, rotation, opacity, radii, geom, binning, img)
+        return g[0], g2d, g[1], g[2], g[3], g[4], g[5], None, None, None, None
+
+
+def backward_raw_depth_native(rs, num_rendered, grad_out_color, depth_mode, grad_depth, grad_alpha, xyz, dc, rest, scaling, rotation,
+                              opacity, radii, geom, binning, img):
+    """lgr_backward_raw_depth: six dense leaf gradients and dL/dmeans2D; grad_depth / grad_alpha [1,H,W] or None (zero)."""
+    lib = capi.load()
+    device = xyz.device
+    P, M = xyz.size(0), 1 + rest.size(1)
+    H, W = grad_out_color.size(1), grad_out_color.size(2)
+    g2d = torch.empty((P, 3), dtype=torch.float32, device=device)
+    g = [torch.empty(t.shape, dtype=torch.float32, device=device) for t in (xyz, dc, rest, scaling, rotation, opacity)]
+    if P != 0:
+        dpix = _f32c(grad_out_color, "grad_out_color")
+        gd = _f32c(grad_depth, "grad_depth") if grad_depth is not None else None
+        ga = _f32c(grad_alpha, "grad_alpha") if grad_alpha is not None else None
+        with torch.cuda.device(device):
+            view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W,
+                                    rs.scale_modifier, rs.sh_degree, False, rs.debug)
+            params, grads = _raw_struct(xyz, dc, rest, scaling, rotation, opacity), _raw_grads_struct(*g)
+            st = lib.lgr_backward_raw_depth(C.byref(view), P, M, int(num_rendered), C.byref(params), radii.data_ptr(), geom.data_ptr(),
+                                            binning.data_ptr(), img.data_ptr(), dpix.data_ptr(), int(depth_mode), capi.ptr(gd), capi.ptr(ga),
+                                            C.byref(grads), g2d.data_ptr(), capi.current_stream_ptr(device))
+        capi.check(st, "lgr_backward_raw_depth")
+    return g, g2d
+
+
+def rasterize_raw_leaves_depth(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity, raster_settings, depth=None,
+                               alpha=False):
+    """(color, radii, depth, alpha) of the fused node: depth [1,H,W] when depth is "z" or "inverse" (else None), alpha [1,H,W] when
+    alpha (else None).  Raises RuntimeError before any launch where the settings have no depth or alpha output."""
+    if depth is not None and depth not in DEPTH_MODES:
+        raise RuntimeError(f"depth={depth!r}: expected None, 'z' or 'inverse'")
+    if raster_settings.f_count:
+        raise RuntimeError("depth / alpha: count mode (raster_settings.f_count) has no depth or alpha output")
+    mode = DEPTH_MODES.get(depth, 0)
+    why = depth_alpha_refusal()
+    if why is not None:
+        raise RuntimeError(f"depth / alpha: {why}")
+    color, radii, d, a = _RasterizeRawLeavesDepth.apply(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity,
+                                                        raster_settings, mode, depth is not None, bool(alpha))
+    return color, radii, (d if depth is not None else None), (a if alpha else None)
 
 
 _side_streams = {}

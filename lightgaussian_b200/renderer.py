@@ -19,7 +19,7 @@ import torch.nn.functional as F
 from . import trace
 
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rasterize_raw_leaves, fused_activations_match_torch,
-                         rest_row_stride, forward_vq_native)
+                         rest_row_stride, forward_vq_native, rasterize_raw_leaves_depth, depth_alpha_refusal, DEPTH_MODES)
 
 _LEAVES = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
 
@@ -116,7 +116,28 @@ def eval_sh_torch(deg: int, sh: torch.Tensor, dirs: torch.Tensor) -> torch.Tenso
     return out
 
 
-def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, f_count, weight=False):
+def _unfused_reason(pc, pipe, override_color) -> str:
+    """why _can_fuse refused, for the depth / alpha error message"""
+    if override_color is not None:
+        return "override_color"
+    if os.environ.get("LGR_FUSED", "1") == "0":
+        return "LGR_FUSED=0"
+    if pipe.convert_SHs_python or pipe.compute_cov3D_python:
+        return "pipe.convert_SHs_python / pipe.compute_cov3D_python"
+    return "a model without GaussianModel's raw float32 CUDA leaves and standard activations (exp / sigmoid / normalize)"
+
+
+def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, f_count, weight=False, depth=None, alpha=False):
+    planes = depth is not None or alpha
+    if planes:
+        # checked before anything is read or launched; a resident VQ model takes the leaf path below (its leaves materialise)
+        if depth is not None and depth not in DEPTH_MODES:
+            raise RuntimeError(f"render(depth={depth!r}): expected None, 'z' or 'inverse'")
+        if not _can_fuse(pc, pipe, override_color):
+            raise RuntimeError(f"render(depth=..., alpha=...) needs the fused path, which {_unfused_reason(pc, pipe, override_color)} rules out")
+        why = depth_alpha_refusal()
+        if why is not None:
+            raise RuntimeError(f"render(depth=..., alpha=...): {why}")
     xyz = pc.get_xyz
     # weight: count mode that also returns the view's fixed-point blending weights (int64 [P], fully written by the forward)
     blend_weight = torch.empty((xyz.shape[0],), dtype=torch.int64, device=xyz.device) if weight else None
@@ -142,6 +163,16 @@ def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_col
         debug=pipe.debug,
         f_count=f_count,
     )
+    if planes:
+        trace.bump("render_depth_alpha")
+        color, radii, d, a = rasterize_raw_leaves_depth(pc._xyz, screenspace_points, pc._features_dc, pc._features_rest, pc._scaling,
+                                                        pc._rotation, pc._opacity, settings, depth, alpha)
+        result = _package((color, radii), screenspace_points, False)
+        if d is not None:
+            result["depth"] = d
+        if a is not None:
+            result["alpha"] = a
+        return result
     store = _resident_store(pc, pipe, override_color)
     if store is not None:
         trace.bump("render_vq_resident")
@@ -204,9 +235,14 @@ def _package(outputs, screenspace_points, f_count, blend_weight=None):
     return result
 
 
-def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):
-    """Render the scene.  Background tensor (bg_color) must be on the GPU."""
-    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, False)
+def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None, *, depth=None, alpha=False):
+    """Render the scene.  Background tensor (bg_color) must be on the GPU.
+    depth="z" / "inverse" adds "depth", and alpha=True adds "alpha", to the result: [1,H,W] float32 planes with gradients to the
+    leaves, sum_i alpha_i*T_i*z_i (z, or 1/z: view-space depth; background 0, not divided by alpha) and 1 - final T (DESIGN.md
+    section 7).  They come from the fused path only: override_color, the pipe's Python flags, LGR_FUSED=0, non-standard activations,
+    deterministic mode, blend mode 1, the view-parallel exchange and LGR_SPARSE_SINGLE=1 raise RuntimeError before any launch.  A
+    resident VQ model asked for them renders from its leaves, which materialise as on any call that needs them."""
+    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, False, depth=depth, alpha=alpha)
 
 
 def count_render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):

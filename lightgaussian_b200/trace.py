@@ -6,6 +6,9 @@ took; with LGR_TRACE=<file> set, the counters below are written to that file (JS
     adamw_steps / adamw_strided_params FusedAdamW.step() calls / row-strided parameters updated in place
     adamw_selective_steps              SelectiveAdamW.step() calls
     unfused_exchange                   view-parallel backward passes that took the dense all-reduce of the unfused node
+    render_depth_alpha                 render(depth=..., alpha=...) calls (the fused node with the depth and alpha planes)
+    raw_backward_depth / raw_backward_plain  backwards of that node through lgr_backward_raw_depth / through lgr_backward_raw, the
+                                       latter when neither plane received a gradient
 Cost when LGR_TRACE is unset: one dict increment per call."""
 from __future__ import annotations
 
