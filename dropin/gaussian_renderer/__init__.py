@@ -11,6 +11,10 @@ except Exception:  # reference checkout not on the path: the name is simply abse
 
 from lightgaussian_b200.renderer import significance_mode as _significance_mode  # noqa: E402
 _significance_mode()   # an unknown LGR_SIGNIFICANCE fails here, not at the first prune
+from lightgaussian_b200.renderer import densify_grad_mode as _densify_grad_mode  # noqa: E402
+if _densify_grad_mode() == "abs" and _os.environ.get("LGR_FUSED_OPTIM", "1") == "0":
+    # LGR_FUSED_OPTIM=0 keeps the class's own add_densification_stats, which would silently accumulate the reference's statistic
+    raise RuntimeError("LGR_DENSIFY_GRAD=abs needs the native densification: it cannot be combined with LGR_FUSED_OPTIM=0")
 if _os.environ.get("LGR_SELECTIVE_ADAM", "0") == "1" and _os.environ.get("LGR_FUSED_OPTIM", "1") == "0":
     raise RuntimeError("LGR_SELECTIVE_ADAM=1 needs the fused optimizer: it cannot be combined with LGR_FUSED_OPTIM=0")
 if GaussianModel is not None and _os.environ.get("LGR_FUSED_OPTIM", "1") != "0":

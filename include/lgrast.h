@@ -233,6 +233,20 @@ int lgr_backward_raw_depth(const lgr_view* view, int P, int M, int num_rendered,
                            const float* dL_dout_color, int depth_mode, const float* dL_ddepth, const float* dL_dalpha,
                            const lgr_raw_grads* grads, float* dL_dmeans2D, void* cuda_stream);
 
+/* ---- absolute-gradient densification statistic (DESIGN.md section 7, "Absolute-gradient densification statistics") ----
+ * lgr_backward_raw_absgrad: the lgr_backward_raw contract (every other output is computed exactly as there) plus
+ * dL_dmeans2D_abs ([P,2] float32 on the device, 8-byte aligned, fully written), the AbsGS / gsplat "absgrad" statistic:
+ *   dL_dmeans2D_abs[i] = (sum_p |dL_p/dmean2D_x(i)|, sum_p |dL_p/dmean2D_y(i)|)
+ * over exactly the pixels p that blend Gaussian i, dL_p/dmean2D being pixel p's term of dL/dmeans2D (the backward run with dL/dpix
+ * zero everywhere except at p), in the units of dL_dmeans2D; 0 for a Gaussian that no pixel blends.  Deterministic mode and the
+ * round-1 blend kernels (lgr_set_blend_mode(1)) have no absgrad: LGR_ERR_INVALID_ARG, nothing launched.  The depth / alpha forward
+ * is recorded on the device only, so a geometry blob from lgr_forward_raw_depth is refused there: every gradient of a visible
+ * Gaussian and every absgrad row is NaN. */
+int lgr_backward_raw_absgrad(const lgr_view* view, int P, int M, int num_rendered, const lgr_raw_params* params,
+                             const int32_t* radii, char* geometry_blob, char* binning_blob, char* image_blob,
+                             const float* dL_dout_color, const lgr_raw_grads* grads, float* dL_dmeans2D,
+                             float* dL_dmeans2D_abs, void* cuda_stream);
+
 /* View-parallel training: for one view dL/dSH[k][c] = basis_k(dir) * dRGB[c] is rank-1 per Gaussian
  * (RAST/cuda_rasterizer/backward.cu:44-97), so ranks exchange dRGB (12 B/Gaussian/view, all-gather) instead of the
  * dense 12*M B/Gaussian gradient, and each rank rebuilds the SUM over views here:

@@ -143,6 +143,10 @@ def load():
         lib.lgr_backward_raw_depth.restype = i32
         lib.lgr_backward_raw_depth.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
                                                i32, vp, vp, C.POINTER(LgrRawGrads), vp, vp]
+        # absolute-gradient densification statistic: lgr_backward_raw's arguments with dL_dmeans2D_abs behind dL_dmeans2D
+        lib.lgr_backward_raw_absgrad.restype = i32
+        lib.lgr_backward_raw_absgrad.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
+                                                 C.POINTER(LgrRawGrads), vp, vp, vp]
         lib.lgr_backward_raw_begin.restype = i32
         lib.lgr_backward_raw_begin.argtypes = [C.POINTER(LgrView), i32, i32, vp, vp, vp, vp, vp, vp, vp]
         lib.lgr_backward_raw_end.restype = i32

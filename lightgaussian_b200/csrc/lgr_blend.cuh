@@ -357,6 +357,18 @@ struct BlendBackWarp {
     float4 d[32];                  // the lanes' dL/dpix (r, g, b) and, DEPTH, dL/ddepth
 };
 
+// The absgrad backward's per-warp buffer (blend_backward_absgrad_kernel): the pair's conic and opacity next to its mean, so the flush
+// can form each source lane's |dL/dmean2D| term from the parked g and the lane's pixel offset.  256 bytes more per warp.
+struct BlendBackWarpAbs : BlendBackWarp {
+    float4 mco[BL_FLUSH];          // per buffered pair: (conic A, conic B, conic C, opacity)
+};
+
+// Where the absgrad backward adds its sums: out[2*id + {0,1}] += (o*0.5W*sum_p |g*(A*dx + B*dy)|, o*0.5H*sum_p |g*(B*dx + C*dy)|).
+struct BlendAbsOut {
+    float* out;    // [P,2]
+    float sx, sy;  // 0.5*W, 0.5*H: the reference's ddelx_dx, ddely_dy
+};
+
 // Deterministic mode: instead of float atomics, each consumer warp parks its 9 sums of every record it blended in this block of
 // shared memory (per stage, warp and record), and the producer warp adds the 8 warps' sums in warp order once the stage is released.
 struct BlendDetStage {
@@ -382,8 +394,12 @@ __host__ __device__ __forceinline__ size_t det_ids_offset(size_t Rn)   // ids_un
 // contract the buffered pairs of one warp and add them to the accumulator records (see the header comment).  DET: `acc` is the
 // warp's slice of BlendDetStage::c for the current stage and bw.mid holds the record's slot in the chunk; plain stores, no atomics.
 // DEPTH: a tenth sum, sum_l w[l] * dL/ddepth[l] = dL/d(depth value), goes to word 9 together with word 8 (one 8-byte reduction).
-template <bool DET = false, bool DEPTH = false>
-__device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, int lane, float ox, float oy, float* __restrict__ acc)
+// ABS (blend_backward_absgrad_kernel): also the two absolute sums of the pair's per-pixel dL/dmean2D terms over the 16 source lanes of
+// each half, from the parked g and each lane's offset d = mean2D - pixel; the lanes that add words 0-3 add them to abs.out with one
+// 8-byte reduction.  `mco` is the warp's BlendBackWarpAbs::mco.
+template <bool DET = false, bool DEPTH = false, bool ABS = false>
+__device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, int lane, float ox, float oy, float* __restrict__ acc,
+                                           const float4* mco = nullptr, BlendAbsOut abs = BlendAbsOut{})
 {
     __syncwarp();
     const int p = lane & 15, h = lane >> 4;
@@ -446,15 +462,45 @@ __device__ __forceinline__ void back_flush(const BlendBackWarp& bw, int nbuf, in
             atomicAdd(rec + 8, s2yy);
         }
     }
+    if (ABS) {
+        // a second pass over the parked g once the nine sums are issued, so that the two absolute sums never share registers with them.
+        // Source lane 16h + 8r + c sits at d = (X - c, Y - r): A*dx + B*dy = u0 - A*c and B*dx + C*dy = v0 - B*c, (u0, v0) at c = 0.
+        // One row of 8 lanes per iteration keeps c an immediate without holding all 16 parked g in registers.
+        const float4 co = mco[p];
+        float ax = 0.f, ay = 0.f;
+#pragma unroll 1
+        for (int r = 0; r < 2; r++) {
+            const float ey = Y - (float)r;
+            const float u0 = fmaf(co.x, X, co.y * ey), v0 = fmaf(co.y, X, co.z * ey);
+#pragma unroll
+            for (int c = 0; c < 8; c++) {
+                const float g = gr[8 * r + c];
+                ax += fabsf(g * fmaf(-co.x, (float)c, u0));
+                ay += fabsf(g * fmaf(-co.y, (float)c, v0));
+            }
+        }
+        ax += __shfl_xor_sync(FULL, ax, 16);
+        ay += __shfl_xor_sync(FULL, ay, 16);
+        if (p < nbuf && h == 0)
+            red_add_v2(abs.out + 2 * (size_t)__float_as_uint(bw.mid[p]), co.w * abs.sx * ax, co.w * abs.sy * ay);
+    }
     __syncwarp();
+}
+
+// back_flush for either warp buffer: only the absgrad kernel's has the conic / opacity rows
+template <bool DET, bool DEPTH, bool ABS, class Warp>
+__device__ __forceinline__ void back_flush_any(const Warp& bw, int nbuf, int lane, float ox, float oy, float* __restrict__ acc, BlendAbsOut abs)
+{
+    if constexpr (ABS) back_flush<false, false, true>(bw, nbuf, lane, ox, oy, acc, bw.mco, abs);
+    else back_flush<DET, DEPTH>(bw, nbuf, lane, ox, oy, acc);
 }
 
 constexpr size_t BL_DET_BYTES = (sizeof(BlendDetStage) + 127) / 128 * 128;
 
-constexpr size_t blend_back_smem_bytes(bool zero_rows = false, bool det = false)
+constexpr size_t blend_back_smem_bytes(bool zero_rows = false, bool det = false, bool abs = false)
 {
-    return (sizeof(BlendRing) + 127) / 128 * 128 + (8 * sizeof(BlendBackWarp) + 127) / 128 * 128 + (det ? BL_DET_BYTES : 0) +
-           (zero_rows ? (size_t)KB_ZERO_BYTES : 0);
+    return (sizeof(BlendRing) + 127) / 128 * 128 + (8 * (abs ? sizeof(BlendBackWarpAbs) : sizeof(BlendBackWarp)) + 127) / 128 * 128 +
+           (det ? BL_DET_BYTES : 0) + (zero_rows ? (size_t)KB_ZERO_BYTES : 0);
 }
 
 // The depth variant's per-pixel inputs (lgr_backward_raw_depth).  `tag` is the HDR_DEPTH value the forward must have left: when the
@@ -473,17 +519,23 @@ struct BlendDepthBack {
 // in ascending unsorted-index order.  The bitmap behind the rows marks the instances that got a row.  No float atomics.
 // DEPTH: the depth and alpha terms (DESIGN section 7): per pixel d.w = dL/ddepth, and D starts at T_final * (bg.dL/dpix - dL/dalpha);
 // per pair cd gains value * dL/ddepth, and the flush adds the tenth sum to record word 9.
-template <bool DET = false, bool DEPTH = false>
-__global__ void __launch_bounds__(BL_THREADS)
-blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_blob, const int* __restrict__ header, int W, int H,
-                           int tiles_x, const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
-                           const float* __restrict__ dL_dpix, float* __restrict__ acc, KbackZeroArgs zero, BlendDepthBack db = BlendDepthBack{})
+// ABS (blend_backward_absgrad_kernel only): also the absolute-gradient densification statistic (back_flush, DESIGN section 7) into
+// abs.out, which the caller cleared.  Like DEPTH it reads header word HDR_DEPTH: a forward that ran the depth blend (db.tag = 0 differs)
+// gets NaN accumulators and NaN absgrad rows.
+template <bool DET, bool DEPTH, bool ABS>
+__device__ __forceinline__ void
+blend_backward_ring_body(const uint2* __restrict__ ranges, const char* __restrict__ binning_blob, const int* __restrict__ header, int W, int H,
+                         int tiles_x, const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
+                         const float* __restrict__ dL_dpix, float* __restrict__ acc, const KbackZeroArgs& zero, const BlendDepthBack& db,
+                         BlendAbsOut abs)
 {
     static_assert(!(DET && DEPTH), "deterministic mode has no depth variant");
+    static_assert(!ABS || (!DET && !DEPTH), "the absgrad backward extends the default kernel only");
+    using Warp = typename std::conditional<ABS, BlendBackWarpAbs, BlendBackWarp>::type;
     extern __shared__ __align__(128) unsigned char blend_dyn_smem[];
     BlendRing& ring = *reinterpret_cast<BlendRing*>(blend_dyn_smem);
-    BlendBackWarp* warps = reinterpret_cast<BlendBackWarp*>(blend_dyn_smem + ((sizeof(BlendRing) + 127) / 128) * 128);
-    unsigned char* behind_warps = reinterpret_cast<unsigned char*>(warps) + (8 * sizeof(BlendBackWarp) + 127) / 128 * 128;
+    Warp* warps = reinterpret_cast<Warp*>(blend_dyn_smem + ((sizeof(BlendRing) + 127) / 128) * 128);
+    unsigned char* behind_warps = reinterpret_cast<unsigned char*>(warps) + (8 * sizeof(Warp) + 127) / 128 * 128;
     BlendDetStage* det = reinterpret_cast<BlendDetStage*>(behind_warps);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x;
@@ -512,12 +564,13 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
     const uint32_t tile_max = ring.tile_max;
     // DEPTH: a forward that ran without depth or in another mode left no (or another) value in record word 11: the records are not read,
     // and NaN accumulators make the misuse show in every gradient (see BlendDepthBack)
-    if (DEPTH && header[HDR_DEPTH] != db.tag) {
+    if ((DEPTH || ABS) && header[HDR_DEPTH] != db.tag) {
         const float nan = __int_as_float(0x7fc00000);
         for (int i = blockIdx.x * BL_THREADS + threadIdx.x; i < db.P; i += gridDim.x * BL_THREADS) {
             float4* rec = reinterpret_cast<float4*>(acc + (size_t)i * ACC_STRIDE);
             rec[0] = rec[1] = make_float4(nan, nan, nan, nan);
             rec[2] = make_float4(nan, nan, 0.f, 0.f);
+            if (ABS) reinterpret_cast<float2*>(abs.out)[i] = make_float2(nan, nan);
         }
         if (zero_rows && threadIdx.x == 8 * 32) bulk_wait_all();   // the zero page must outlive the stores that read it
         return;
@@ -602,7 +655,7 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
     }
 
     // ===== consumers =====
-    BlendBackWarp& bw = warps[warp];
+    Warp& bw = warps[warp];
     float pxf = (float)px, pyf = (float)py;
     const float rx0 = (float)sx0, rx1 = (float)min(sx0 + 7, W - 1), ry0 = (float)sy0, ry1 = (float)min(sy0 + 3, H - 1);
     const float T_final = inside ? final_T[pix] : 0.f;
@@ -677,10 +730,11 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
                     bw.mid[nbuf] = DET ? __uint_as_float((uint32_t)j) : q2.y;
                     bw.mgx[nbuf] = q0.x;
                     bw.mgy[nbuf] = q0.y;
+                    if constexpr (ABS) bw.mco[nbuf] = make_float4(q0.z, q0.w, q1.x, q1.y);
                 }
                 if (DET) wrote |= 1u << j;
                 if (++nbuf == BL_FLUSH) {
-                    back_flush<DET, DEPTH>(bw, nbuf, lane, rx0, ry0, parked);
+                    back_flush_any<DET, DEPTH, ABS>(bw, nbuf, lane, rx0, ry0, parked, abs);
                     nbuf = 0;
                 }
             }
@@ -694,7 +748,30 @@ blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restr
         __syncwarp();
         if (lane == 0) mbar_arrive(&ring.empty[s]);
     }
-    if (!DET && nbuf) back_flush<false, DEPTH>(bw, nbuf, lane, rx0, ry0, acc);
+    if (!DET && nbuf) back_flush_any<false, DEPTH, ABS>(bw, nbuf, lane, rx0, ry0, acc, abs);
+}
+
+template <bool DET = false, bool DEPTH = false>
+__global__ void __launch_bounds__(BL_THREADS)
+blend_backward_ring_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_blob, const int* __restrict__ header, int W, int H,
+                           int tiles_x, const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
+                           const float* __restrict__ dL_dpix, float* __restrict__ acc, KbackZeroArgs zero, BlendDepthBack db = BlendDepthBack{})
+{
+    blend_backward_ring_body<DET, DEPTH, false>(ranges, binning_blob, header, W, H, tiles_x, bg, final_T, n_contrib, dL_dpix, acc, zero, db,
+                                                BlendAbsOut{});
+}
+
+// The default kernel plus the absolute-gradient densification statistic (lgr_backward_raw_absgrad): absgrad[P,2] (cleared by the
+// caller) gains, per (warp, Gaussian), o*(0.5W, 0.5H) times the sums over the warp's pixels of |g*(A*dx + B*dy)| and |g*(B*dx + C*dy)|.
+// Four blocks per SM like the default kernel: 56 registers or fewer.
+__global__ void __launch_bounds__(BL_THREADS, 4)
+blend_backward_absgrad_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_blob, const int* __restrict__ header, int W, int H,
+                              int tiles_x, const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
+                              const float* __restrict__ dL_dpix, float* __restrict__ acc, KbackZeroArgs zero, float* __restrict__ absgrad, int P)
+{
+    const BlendDepthBack db = {nullptr, nullptr, 0, P};   // tag 0: the forward must not have run the depth blend
+    blend_backward_ring_body<false, false, true>(ranges, binning_blob, header, W, H, tiles_x, bg, final_T, n_contrib, dL_dpix, acc, zero, db,
+                                                 BlendAbsOut{absgrad, 0.5f * (float)W, 0.5f * (float)H});
 }
 
 // ---- deterministic mode, across tiles: the Gaussian of depth rank k owns the unsorted instances [offsets[k-1], offsets[k]) (emit

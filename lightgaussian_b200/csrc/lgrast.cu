@@ -1913,8 +1913,11 @@ thread_local bool t_rows_zeroed = false;
 
 // stage 1 of the raw backward: clear the accumulators, blend backward, optionally extract this view's dL/dRGB.  db: the depth variant
 // of the blend backward (lgr_backward_raw_depth; the caller refused deterministic mode and blend mode 1)
+// absgrad: the absgrad variant of the blend backward (lgr_backward_raw_absgrad; the caller refused deterministic mode and blend mode 1)
+// adds the statistic into absgrad[P,2], which this function clears
 static int backward_raw_begin_impl(const lgr_view* v, int P, int num_rendered, const int32_t* radii, char* geometry_blob, char* binning_blob,
-                                   char* image_blob, const float* dL_dout_color, float* d_rgb, void* cuda_stream, const BlendDepthBack* db)
+                                   char* image_blob, const float* dL_dout_color, float* d_rgb, void* cuda_stream, const BlendDepthBack* db,
+                                   float* absgrad = nullptr)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     if (P == 0) return LGR_OK;
@@ -1938,6 +1941,7 @@ static int backward_raw_begin_impl(const lgr_view* v, int P, int num_rendered, c
     } else {
         ProfScope ps(ST_MEMSET, stream);
         LGR_CUDA_TRY(cudaMemsetAsync(geo.grad_acc, 0, sizeof(float) * ACC_STRIDE * (size_t)P, stream));
+        if (absgrad) LGR_CUDA_TRY(cudaMemsetAsync(absgrad, 0, sizeof(float) * 2 * (size_t)P, stream));
     }
     if (num_rendered > 0 && !g_det) {
         ProfScope ps(ST_BLEND_BWD, stream);
@@ -1948,7 +1952,13 @@ static int backward_raw_begin_impl(const lgr_view* v, int P, int num_rendered, c
             const KbackZeroArgs zr = t_zero_req;
             t_zero_req.P = 0;
             const size_t bsmem = blend_back_smem_bytes(zr.P > 0);
-            if (db) {
+            if (absgrad) {
+                LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_absgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  (int)blend_back_smem_bytes(true, false, true)));
+                blend_backward_absgrad_kernel<<<gx * gy, BL_THREADS, blend_back_smem_bytes(zr.P > 0, false, true), stream>>>(
+                    img.ranges, binning_blob, geo.num_rendered, W, H, gx, v->background, img.final_T, img.n_contrib, dL_dout_color,
+                    geo.grad_acc, zr, absgrad, P);
+            } else if (db) {
                 LGR_CUDA_TRY(cudaFuncSetAttribute(blend_backward_ring_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                   (int)blend_back_smem_bytes(true)));
                 blend_backward_ring_kernel<false, true><<<gx * gy, BL_THREADS, bsmem, stream>>>(img.ranges, binning_blob, geo.num_rendered, W, H, gx,
@@ -2081,7 +2091,7 @@ int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_pa
 
 static int backward_raw_impl(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
                              char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, const lgr_raw_grads* grads,
-                             float* dL_dmeans2D, void* cuda_stream, const BlendDepthBack* db, const RawDepth* rd)
+                             float* dL_dmeans2D, void* cuda_stream, const BlendDepthBack* db, const RawDepth* rd, float* absgrad = nullptr)
 {
     t_zero_req.P = 0;
     t_rows_zeroed = false;
@@ -2095,7 +2105,8 @@ static int backward_raw_impl(const lgr_view* v, int P, int M, int num_rendered, 
         z.d_xyz = grads->xyz; z.d_dc = grads->features_dc; z.d_rest = grads->features_rest; z.d_scaling = grads->scaling;
         z.d_rotation = grads->rotation; z.d_opacity = grads->opacity; z.dL_dmeans2D = dL_dmeans2D;
     }
-    const int st = backward_raw_begin_impl(v, P, num_rendered, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, nullptr, cuda_stream, db);
+    const int st = backward_raw_begin_impl(v, P, num_rendered, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, nullptr, cuda_stream, db,
+                                           absgrad);
     t_zero_req.P = 0;
     if (st != LGR_OK) { t_rows_zeroed = false; return st; }
     return backward_raw_end_impl(v, P, M, params, radii, geometry_blob, grads, dL_dmeans2D, 0, P, cuda_stream, rd);
@@ -2170,6 +2181,31 @@ int lgr_backward_raw_depth(const lgr_view* v, int P, int M, int num_rendered, co
     const RawDepth rd = {carve_geometry(geometry_blob, (size_t)P, false).depth, depth_mode};
     return backward_raw_impl(v, P, M, num_rendered, params, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dmeans2D,
                              cuda_stream, &db, &rd);
+}
+
+// ---- absolute-gradient densification statistic (DESIGN section 7) ----
+int lgr_backward_raw_absgrad(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
+                             char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, const lgr_raw_grads* grads,
+                             float* dL_dmeans2D, float* dL_dmeans2D_abs, void* cuda_stream)
+{
+    if (g_det) {
+        g_last_error = "lgr_backward_raw_absgrad: deterministic mode has no absgrad output (it needs fixed-order sums)";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (g_blend_mode != 0) {
+        g_last_error = "lgr_backward_raw_absgrad: absgrad needs the ring blend kernels; lgr_set_blend_mode(1) has no absgrad output";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (P == 0) return LGR_OK;
+    if (P < 0 || !dL_dmeans2D_abs || ((uintptr_t)dL_dmeans2D_abs & 7)) {
+        g_last_error = "lgr_backward_raw_absgrad: dL_dmeans2D_abs must be an 8-byte aligned [P,2] float32 device array";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (num_rendered <= 0) {   // no pair: the blend backward does not run, so the statistic is cleared here
+        LGR_CUDA_TRY(cudaMemsetAsync(dL_dmeans2D_abs, 0, sizeof(float) * 2 * (size_t)P, static_cast<cudaStream_t>(cuda_stream)));
+    }
+    return backward_raw_impl(v, P, M, num_rendered, params, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dmeans2D,
+                             cuda_stream, nullptr, nullptr, num_rendered > 0 ? dL_dmeans2D_abs : nullptr);
 }
 
 // ---- sparse view-parallel exchange (lgr_sparse.cuh) ----

@@ -20,6 +20,7 @@ import torch
 
 from . import capi, rasterizer, trace
 from .optim import _GROUP_ATTR
+from .renderer import densify_grad_mode
 
 _ROLE = {"xyz": capi.DENSIFY_XYZ, "scaling": capi.DENSIFY_SCALING}
 _ROW_SHAPE = {"xyz": (3,), "scaling": (3,), "rotation": (4,), "opacity": (1,)}
@@ -47,7 +48,12 @@ def _dense_f32(t, device, shape) -> bool:
 def add_densification_stats(gaussians, viewspace_point_tensor, update_filter):
     """GaussianModel.add_densification_stats (:784-788).  With the view-parallel densification exchange on
     (parallel.enable_gradient_exchange(world > 1, densification=True)) it adds every rank's view of the step, in rank order, on every
-    rank: from the slots of the step's sparse exchange when its backward published them, else through one all-gather."""
+    rank: from the slots of the step's sparse exchange when its backward published them, else through one all-gather.
+    With LGR_DENSIFY_GRAD=abs (read at each call) it adds ||absgrad[f]|| instead, from the `absgrad` [P,2] that render()'s backward
+    set on the tensor; it raises where that statistic is missing or cannot be added natively (no fall-back to the class's method)."""
+    if densify_grad_mode() == "abs":
+        _add_absgrad_stats(gaussians, viewspace_point_tensor, update_filter)
+        return
     grad = getattr(viewspace_point_tensor, "grad", None)
     accum, denom = getattr(gaussians, "xyz_gradient_accum", None), getattr(gaussians, "denom", None)
     P = accum.shape[0] if isinstance(accum, torch.Tensor) else -1
@@ -75,6 +81,30 @@ def add_densification_stats(gaussians, viewspace_point_tensor, update_filter):
     lib = capi.load()
     with torch.cuda.device(device):
         capi.check(lib.lgr_densify_stats(P, grad.data_ptr(), grad.stride(0), update_filter.data_ptr(), accum.data_ptr(), denom.data_ptr(),
+                                         capi.current_stream_ptr(device)), "lgr_densify_stats")
+
+
+def _add_absgrad_stats(gaussians, viewspace_point_tensor, update_filter):
+    """xyz_gradient_accum[f] += ||absgrad[f]||, denom[f] += 1 through lgr_densify_stats (row stride 2)"""
+    absgrad = getattr(viewspace_point_tensor, "absgrad", None)
+    if absgrad is None:
+        raise RuntimeError("LGR_DENSIFY_GRAD=abs: the view-space tensor has no .absgrad; render it with LGR_DENSIFY_GRAD=abs set and "
+                           "gradients enabled, and call backward first")
+    if rasterizer.densification_exchange():
+        raise RuntimeError("LGR_DENSIFY_GRAD=abs: the view-parallel densification exchange has no absgrad")
+    accum, denom = getattr(gaussians, "xyz_gradient_accum", None), getattr(gaussians, "denom", None)
+    P = accum.shape[0] if isinstance(accum, torch.Tensor) else -1
+    device = absgrad.device
+    if not (_dense_f32(absgrad, device, (P, 2)) and isinstance(update_filter, torch.Tensor) and update_filter.dtype == torch.bool
+            and update_filter.device == device and update_filter.is_contiguous() and tuple(update_filter.shape) == (P,)
+            and _dense_f32(accum, device, (P, 1)) and _dense_f32(denom, device, (P, 1))):
+        raise RuntimeError("LGR_DENSIFY_GRAD=abs needs a float32 CUDA absgrad [P,2], a contiguous bool filter [P] and float32 [P,1] "
+                           "xyz_gradient_accum / denom on the same device")
+    trace.bump("densify_stats_native")
+    trace.bump("densify_stats_absgrad")
+    lib = capi.load()
+    with torch.cuda.device(device):
+        capi.check(lib.lgr_densify_stats(P, absgrad.data_ptr(), 2, update_filter.data_ptr(), accum.data_ptr(), denom.data_ptr(),
                                          capi.current_stream_ptr(device)), "lgr_densify_stats")
 
 

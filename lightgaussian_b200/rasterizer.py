@@ -520,6 +520,74 @@ class _RasterizeRawLeaves(torch.autograd.Function):
         return g[0], g2d, g[1], g[2], g[3], g[4], g[5], None
 
 
+class _RasterizeRawLeavesAbs(torch.autograd.Function):
+    """render()'s fused node under LGR_DENSIFY_GRAD=abs: _RasterizeRawLeaves whose backward goes through lgr_backward_raw_absgrad and
+    sets `means2D.absgrad` ([P,2] float32, the sum over pixels of each pixel's |dL/dmean2D| term).  means2D.grad is unchanged."""
+
+    @staticmethod
+    def forward(ctx, xyz, means2D, dc, rest, scaling, rotation, opacity, raster_settings):
+        color, radii = _RasterizeRawLeaves.forward(ctx, xyz, means2D, dc, rest, scaling, rotation, opacity, raster_settings)
+        ctx.means2D = means2D   # render()'s screen-space placeholder, which the caller reads .absgrad from
+        return color, radii
+
+    @staticmethod
+    def backward(ctx, grad_out_color, _):
+        xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img = ctx.saved_tensors
+        capi.set_deterministic(ctx.deterministic)   # refused by the forward; the library refuses it again if the flag changed since
+        trace.bump("raw_backward_absgrad")
+        g, g2d, absgrad = backward_raw_absgrad_native(ctx.raster_settings, ctx.num_rendered, grad_out_color, xyz, dc, rest, scaling,
+                                                      rotation, opacity, radii, geom, binning, img)
+        ctx.means2D.absgrad = absgrad
+        return g[0], g2d, g[1], g[2], g[3], g[4], g[5], None
+
+
+def absgrad_refusal() -> str | None:
+    """Why the fused node cannot compute the absolute-gradient statistic under the current settings, or None.  Checked before any
+    launch."""
+    if capi.deterministic_requested():
+        return "deterministic mode (LGR_DETERMINISTIC=1 or torch.use_deterministic_algorithms) has no absgrad (it needs fixed-order sums)"
+    if capi.blend_mode() != 0:
+        return "blend mode 1 (the round-1 blend kernels) has no absgrad"
+    if _exchange["world"] > 1:
+        return "the view-parallel gradient exchange has no absgrad backward"
+    if _os.environ.get("LGR_SPARSE_SINGLE", "0") == "1":
+        return "LGR_SPARSE_SINGLE=1 (the sparse single-GPU backward) has no absgrad backward"
+    return None
+
+
+def backward_raw_absgrad_native(rs, num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img):
+    """lgr_backward_raw_absgrad: six dense leaf gradients, dL/dmeans2D [P,3] and absgrad [P,2]."""
+    lib = capi.load()
+    device = xyz.device
+    P, M = xyz.size(0), 1 + rest.size(1)
+    H, W = grad_out_color.size(1), grad_out_color.size(2)
+    g2d = torch.empty((P, 3), dtype=torch.float32, device=device)
+    absgrad = torch.empty((P, 2), dtype=torch.float32, device=device)
+    g = [torch.empty(t.shape, dtype=torch.float32, device=device) for t in (xyz, dc, rest, scaling, rotation, opacity)]
+    if P != 0:
+        dpix = _f32c(grad_out_color, "grad_out_color")
+        with torch.cuda.device(device):
+            view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W,
+                                    rs.scale_modifier, rs.sh_degree, False, rs.debug)
+            params, grads = _raw_struct(xyz, dc, rest, scaling, rotation, opacity), _raw_grads_struct(*g)
+            st = lib.lgr_backward_raw_absgrad(C.byref(view), P, M, int(num_rendered), C.byref(params), radii.data_ptr(), geom.data_ptr(),
+                                              binning.data_ptr(), img.data_ptr(), dpix.data_ptr(), C.byref(grads), g2d.data_ptr(),
+                                              absgrad.data_ptr(), capi.current_stream_ptr(device))
+        capi.check(st, "lgr_backward_raw_absgrad")
+    return g, g2d, absgrad
+
+
+def rasterize_raw_leaves_absgrad(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity, raster_settings):
+    """(color, radii) of the fused node whose backward also sets means2D.absgrad.  Raises RuntimeError before any launch where the
+    settings have no absgrad."""
+    if raster_settings.f_count:
+        raise RuntimeError("LGR_DENSIFY_GRAD=abs: count mode (raster_settings.f_count) has no absgrad")
+    why = absgrad_refusal()
+    if why is not None:
+        raise RuntimeError(f"LGR_DENSIFY_GRAD=abs: {why}")
+    return _RasterizeRawLeavesAbs.apply(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity, raster_settings)
+
+
 DEPTH_MODES = {"z": 1, "inverse": 2}
 
 

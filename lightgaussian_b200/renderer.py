@@ -19,7 +19,8 @@ import torch.nn.functional as F
 from . import trace
 
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rasterize_raw_leaves, fused_activations_match_torch,
-                         rest_row_stride, forward_vq_native, rasterize_raw_leaves_depth, depth_alpha_refusal, DEPTH_MODES)
+                         rest_row_stride, forward_vq_native, rasterize_raw_leaves_depth, depth_alpha_refusal, DEPTH_MODES,
+                         rasterize_raw_leaves_absgrad, absgrad_refusal)
 
 _LEAVES = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
 
@@ -35,14 +36,27 @@ def significance_mode() -> str:
     return mode
 
 
+DENSIFY_GRAD_MODES = ("grad", "abs")
+
+
+def densify_grad_mode() -> str:
+    """LGR_DENSIFY_GRAD, read at call time: "grad" (unset; the reference's ||sum_p dL_p/dmean2D||) or "abs" (AbsGS / gsplat absgrad:
+    render() sets viewspace_points.absgrad = sum_p |dL_p/dmean2D| and add_densification_stats accumulates its norm)."""
+    mode = os.environ.get("LGR_DENSIFY_GRAD", "grad")
+    if mode not in DENSIFY_GRAD_MODES:
+        raise RuntimeError(f"LGR_DENSIFY_GRAD={mode!r}: expected one of {', '.join(DENSIFY_GRAD_MODES)}")
+    return mode
+
+
 def weight_score(blend_weight_fx: torch.Tensor) -> torch.Tensor:
     """float32 score of int64 fixed-point blending weights: float32(float64(fx) * 2^-32)."""
     return (blend_weight_fx.to(torch.float64) * WEIGHT_SCALE).to(torch.float32)
 
 
-def _can_fuse(pc, pipe, override_color) -> bool:
+def _can_fuse(pc, pipe, override_color, dense_copies=False) -> bool:
     """The fused path needs GaussianModel-style raw leaves with the standard activations
-    (scene/gaussian_model.py:35-43: exp / sigmoid / normalize) and the default pipeline flags."""
+    (scene/gaussian_model.py:35-43: exp / sigmoid / normalize) and the default pipeline flags.  dense_copies: the caller hands
+    non-contiguous leaves to the fused node as contiguous copies (_dense_leaves), so their layout does not matter."""
     if os.environ.get("LGR_FUSED", "1") == "0" or override_color is not None:
         return False
     if pipe.convert_SHs_python or pipe.compute_cov3D_python:
@@ -58,16 +72,27 @@ def _can_fuse(pc, pipe, override_color) -> bool:
     t = pc._xyz
     # every leaf dense, except that _features_rest may be a row-strided view: the distillation student's
     # `_features_rest[:, :8, :]` (scene/gaussian_model.py:129-136) is read in place through its row stride
-    if not (t.is_cuda and all(getattr(pc, n).dtype == torch.float32 and (getattr(pc, n).is_contiguous() or n == "_features_rest")
-                              for n in _LEAVES)):
+    if not (t.is_cuda and all(getattr(pc, n).dtype == torch.float32
+                              and (dense_copies or getattr(pc, n).is_contiguous() or n == "_features_rest") for n in _LEAVES)):
         return False
     if pc._features_rest.dim() != 3 or pc._features_dc.shape[1] != 1 or pc._features_rest.shape[1] < 1:
         return False
-    if not pc._features_rest.is_contiguous() and rest_row_stride(pc._features_rest) == 0:
+    if not dense_copies and not pc._features_rest.is_contiguous() and rest_row_stride(pc._features_rest) == 0:
         return False
     if (pc.active_sh_degree + 1) ** 2 > 1 + pc._features_rest.shape[1]:
         return False
     return fused_activations_match_torch(t.device)
+
+def _dense_leaves(pc):
+    """the six leaves for the fused node, each non-contiguous one (create_from_pcd's permuted _xyz) as a contiguous copy whose gradient
+    autograd routes back to the leaf; a row-strided _features_rest the kernels read in place stays as it is"""
+    out = []
+    for n in _LEAVES:
+        t = getattr(pc, n)
+        keep = t.is_contiguous() or (n == "_features_rest" and rest_row_stride(t) != 0)
+        out.append(t if keep else t.contiguous())
+    return out
+
 
 def _resident_store(pc, pipe, override_color):
     """The resident VQ store of `pc` (vqresident.py) when this call can render the compressed model in place: a forward without
@@ -129,6 +154,16 @@ def _unfused_reason(pc, pipe, override_color) -> str:
 
 def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, f_count, weight=False, depth=None, alpha=False):
     planes = depth is not None or alpha
+    # LGR_DENSIFY_GRAD=abs: the training render's backward also produces viewspace_points.absgrad; checked before anything is read
+    absgrad = not f_count and densify_grad_mode() == "abs" and torch.is_grad_enabled()
+    if absgrad:
+        if planes:
+            raise RuntimeError("LGR_DENSIFY_GRAD=abs cannot be combined with render(depth=..., alpha=...)")
+        if not _can_fuse(pc, pipe, override_color, dense_copies=True):
+            raise RuntimeError(f"LGR_DENSIFY_GRAD=abs needs the fused path, which {_unfused_reason(pc, pipe, override_color)} rules out")
+        why = absgrad_refusal()
+        if why is not None:
+            raise RuntimeError(f"LGR_DENSIFY_GRAD=abs: {why}")
     if planes:
         # checked before anything is read or launched; a resident VQ model takes the leaf path below (its leaves materialise)
         if depth is not None and depth not in DEPTH_MODES:
@@ -163,6 +198,12 @@ def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_col
         debug=pipe.debug,
         f_count=f_count,
     )
+    if absgrad:
+        trace.bump("render_fused")
+        trace.bump("render_absgrad")
+        xyz_, dc, rest, scaling, rotation, opacity = _dense_leaves(pc)
+        outputs = rasterize_raw_leaves_absgrad(xyz_, screenspace_points, dc, rest, scaling, rotation, opacity, settings)
+        return _package(outputs, screenspace_points, f_count)
     if planes:
         trace.bump("render_depth_alpha")
         color, radii, d, a = rasterize_raw_leaves_depth(pc._xyz, screenspace_points, pc._features_dc, pc._features_rest, pc._scaling,
@@ -241,7 +282,10 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     leaves, sum_i alpha_i*T_i*z_i (z, or 1/z: view-space depth; background 0, not divided by alpha) and 1 - final T (DESIGN.md
     section 7).  They come from the fused path only: override_color, the pipe's Python flags, LGR_FUSED=0, non-standard activations,
     deterministic mode, blend mode 1, the view-parallel exchange and LGR_SPARSE_SINGLE=1 raise RuntimeError before any launch.  A
-    resident VQ model asked for them renders from its leaves, which materialise as on any call that needs them."""
+    resident VQ model asked for them renders from its leaves, which materialise as on any call that needs them.
+    With LGR_DENSIFY_GRAD=abs (read at each call) and gradients enabled, the backward also sets `viewspace_points.absgrad` ([P,2], the
+    sum over pixels of each pixel's |dL/dmean2D| term, DESIGN.md section 7) for add_densification_stats; the same paths, depth= and
+    alpha= then raise RuntimeError before any launch.  Without gradients the variable changes nothing."""
     return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, False, depth=depth, alpha=alpha)
 
 

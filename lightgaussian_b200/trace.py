@@ -9,6 +9,9 @@ took; with LGR_TRACE=<file> set, the counters below are written to that file (JS
     render_depth_alpha                 render(depth=..., alpha=...) calls (the fused node with the depth and alpha planes)
     raw_backward_depth / raw_backward_plain  backwards of that node through lgr_backward_raw_depth / through lgr_backward_raw, the
                                        latter when neither plane received a gradient
+    render_absgrad / raw_backward_absgrad  render() calls through the fused node that also computes the absolute-gradient
+                                       densification statistic (LGR_DENSIFY_GRAD=abs) / its backwards (lgr_backward_raw_absgrad)
+    densify_stats_absgrad              add_densification_stats calls that added ||absgrad|| (LGR_DENSIFY_GRAD=abs)
 Cost when LGR_TRACE is unset: one dict increment per call."""
 from __future__ import annotations
 
