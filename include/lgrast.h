@@ -247,6 +247,30 @@ int lgr_backward_raw_absgrad(const lgr_view* view, int P, int M, int num_rendere
                              const float* dL_dout_color, const lgr_raw_grads* grads, float* dL_dmeans2D,
                              float* dL_dmeans2D_abs, void* cuda_stream);
 
+/* ---- camera gradients (DESIGN.md section 7, "Camera gradients") ----
+ * lgr_backward_raw_camera: the lgr_backward_raw_depth contract (depth_mode 0 with dL_ddepth and dL_dalpha NULL is lgr_backward_raw;
+ * every other output is computed exactly as there) plus the loss gradient with respect to the three camera arrays of `view`:
+ *   dL_dviewmatrix [16], dL_dprojmatrix [16], dL_dcampos [3]: float32 device arrays, fully written.
+ * With V = viewmatrix, Pm = projmatrix, c = campos and p = (x, y, z, 1) a Gaussian's world mean, summed over every Gaussian the
+ * per-Gaussian backward differentiates:
+ *   dL/dV[4r+k]  = p_r dL/dt_k (t_k = sum_r p_r V[4r+k], k < 3: the camera-space mean, through the J path of the 2D covariance with the
+ *                  forward's 1.3 tan(fov) clamp, and the depth plane) plus, for r, k < 3, (J^T dL/dT)[k][r] (T = J W, W[a][k] = V[4k+a])
+ *   dL/dPm[4r+k] = p_r dL/dh_k, k in {0, 1, 3} (h_k = sum_r p_r Pm[4r+k]; ndc = (h_0, h_1) / (h_3 + 1e-7))
+ *   dL/dc        = minus the sum of the view-direction terms of the SH backward
+ * V[4r+3] and Pm[4r+2] are never read: those eight entries are 0.  The intrinsics (tan_fovx / tan_fovy) get no gradient.  All three
+ * outputs are 0 when P == 0 or nothing is differentiated.  Deterministic mode runs the dense per-Gaussian kernel, whose partial sums
+ * have a fixed order: two calls on one forward return bit-identical camera gradients.  Otherwise the compacted kernel's list is in
+ * block-arrival order and the camera gradients may differ between runs in the last bits.  `workspace`: device memory of at least
+ * lgr_camera_grad_workspace_bytes(P) bytes, 4-byte aligned.  With a depth or alpha plane, deterministic mode and the round-1 blend
+ * kernels are refused as by lgr_backward_raw_depth (LGR_ERR_INVALID_ARG, nothing launched); a geometry blob from a forward in another
+ * depth mode gives NaN camera gradients along with the NaN leaf gradients. */
+size_t lgr_camera_grad_workspace_bytes(int P);
+int lgr_backward_raw_camera(const lgr_view* view, int P, int M, int num_rendered, const lgr_raw_params* params,
+                            const int32_t* radii, char* geometry_blob, char* binning_blob, char* image_blob,
+                            const float* dL_dout_color, int depth_mode, const float* dL_ddepth, const float* dL_dalpha,
+                            const lgr_raw_grads* grads, float* dL_dmeans2D, float* dL_dviewmatrix, float* dL_dprojmatrix,
+                            float* dL_dcampos, void* workspace, size_t workspace_bytes, void* cuda_stream);
+
 /* View-parallel training: for one view dL/dSH[k][c] = basis_k(dir) * dRGB[c] is rank-1 per Gaussian
  * (RAST/cuda_rasterizer/backward.cu:44-97), so ranks exchange dRGB (12 B/Gaussian/view, all-gather) instead of the
  * dense 12*M B/Gaussian gradient, and each rank rebuilds the SUM over views here:

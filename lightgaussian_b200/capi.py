@@ -147,6 +147,13 @@ def load():
         lib.lgr_backward_raw_absgrad.restype = i32
         lib.lgr_backward_raw_absgrad.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
                                                  C.POINTER(LgrRawGrads), vp, vp, vp]
+        # camera gradients: lgr_backward_raw_depth's arguments with (dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace,
+        # workspace_bytes) behind dL_dmeans2D
+        lib.lgr_camera_grad_workspace_bytes.restype = C.c_size_t
+        lib.lgr_camera_grad_workspace_bytes.argtypes = [i32]
+        lib.lgr_backward_raw_camera.restype = i32
+        lib.lgr_backward_raw_camera.argtypes = [C.POINTER(LgrView), i32, i32, i32, C.POINTER(LgrRawParams), vp, vp, vp, vp, vp,
+                                                i32, vp, vp, C.POINTER(LgrRawGrads), vp, vp, vp, vp, vp, C.c_size_t, vp]
         lib.lgr_backward_raw_begin.restype = i32
         lib.lgr_backward_raw_begin.argtypes = [C.POINTER(LgrView), i32, i32, vp, vp, vp, vp, vp, vp, vp]
         lib.lgr_backward_raw_end.restype = i32

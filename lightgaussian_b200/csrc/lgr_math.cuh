@@ -360,8 +360,11 @@ struct GradIn {
 };
 
 // conic gradient -> dL/dcov3D[6] and the covariance part of dL/dmean3D.  cov3D = forward's 6 floats.
+// dcam (optional, camera gradients): [0..2] = dL/dt, the camera-space mean gradient of the J path (clamp masks applied);
+// [3 + 3r + k] = dL/dV[4r + k] for r, k < 3 through T = J W, i.e. (J^T dT)[k][r] with J at the clamped tx, ty.  When dcam is NULL
+// the function is the leaf-only backward it always was.
 LGR_HD void cov2d_backward(float px, float py, float pz, const float* v, const float* c3, float fx, float fy, float tanx,
-                           float tany, float dA, float dB, float dC, float* dcov, float* dmean)
+                           float tany, float dA, float dB, float dC, float* dcov, float* dmean, float* dcam = nullptr)
 {
     Ewa e;
     ewa_setup(px, py, pz, v, fx, fy, tanx, tany, e);
@@ -407,10 +410,22 @@ LGR_HD void cov2d_backward(float px, float py, float pz, const float* v, const f
     dmean[0] = v[0] * dtx + v[1] * dty + v[2] * dtz;
     dmean[1] = v[4] * dtx + v[5] * dty + v[6] * dtz;
     dmean[2] = v[8] * dtx + v[9] * dty + v[10] * dtz;
+    if (dcam) {
+        // T[i][r] = sum_k J[i][k] V[4r + k] with J = [[j00, 0, j02], [0, j11, j12]] (ewa_setup)
+        const float j00 = fx * iz, j02 = -fx * e.tx * iz2, j11 = fy * iz, j12 = -fy * e.ty * iz2;
+        const float dT0[3] = {dT00, dT01, dT02}, dT1[3] = {dT10, dT11, dT12};
+        dcam[0] = dtx; dcam[1] = dty; dcam[2] = dtz;
+        for (int r = 0; r < 3; r++) {
+            dcam[3 + 3 * r + 0] = j00 * dT0[r];
+            dcam[3 + 3 * r + 1] = j11 * dT1[r];
+            dcam[3 + 3 * r + 2] = j02 * dT0[r] + j12 * dT1[r];
+        }
+    }
 }
 
 // screen-space mean gradient -> 3D mean (RAST/cuda_rasterizer/backward.cu:370-387); accumulates into dmean.
-LGR_HD void mean2d_backward(float px, float py, float pz, const float* proj, float g2x, float g2y, float* dmean)
+// dh (optional, camera gradients): dL/dh for the homogeneous mean h = (h_x, h_y, h_w), ndc = (h_x, h_y) / (h_w + 1e-7).
+LGR_HD void mean2d_backward(float px, float py, float pz, const float* proj, float g2x, float g2y, float* dmean, float* dh = nullptr)
 {
     const float hw = proj[3] * px + proj[7] * py + proj[11] * pz + proj[15];
     const float mw = 1.0f / (hw + 0.0000001f);
@@ -419,13 +434,21 @@ LGR_HD void mean2d_backward(float px, float py, float pz, const float* proj, flo
     dmean[0] += (proj[0] * mw - proj[3] * mul1) * g2x + (proj[1] * mw - proj[3] * mul2) * g2y;
     dmean[1] += (proj[4] * mw - proj[7] * mul1) * g2x + (proj[5] * mw - proj[7] * mul2) * g2y;
     dmean[2] += (proj[8] * mw - proj[11] * mul1) * g2x + (proj[9] * mw - proj[11] * mul2) * g2y;
+    if (dh) {
+        const float hx = proj[0] * px + proj[4] * py + proj[8] * pz + proj[12];
+        const float hy = proj[1] * px + proj[5] * py + proj[9] * pz + proj[13];
+        dh[0] = g2x * mw;
+        dh[1] = g2y * mw;
+        dh[2] = -(g2x * hx + g2y * hy) * (mw * mw);
+    }
 }
 
 // SH backward (RAST/cuda_rasterizer/backward.cu:20-139).  dRGB already masked by the clamp bits.
 // Calls store(k, c, value) for every k < (deg+1)^2 and accumulates the view-direction term into dmean.
+// ddir (optional, camera gradients): receives that view-direction term itself; dL/dcampos is its negative.
 template <typename ShLoad, typename ShStore>
 LGR_HD void sh_backward(int deg, ShLoad sh, ShStore store, float px, float py, float pz, const float* cam, const float* dRGB,
-                        float* dmean)
+                        float* dmean, float* ddir = nullptr)
 {
     const float ox = px - cam[0], oy = py - cam[1], oz = pz - cam[2];
     const float s2 = ox * ox + oy * oy + oz * oz;
@@ -475,6 +498,11 @@ LGR_HD void sh_backward(int deg, ShLoad sh, ShStore store, float px, float py, f
     dmean[0] += ((s2 - ox * ox) * ddx - oy * ox * ddy - oz * ox * ddz) * inv32;
     dmean[1] += (-ox * oy * ddx + (s2 - oy * oy) * ddy - oz * oy * ddz) * inv32;
     dmean[2] += (-ox * oz * ddx - oy * oz * ddy + (s2 - oz * oz) * ddz) * inv32;
+    if (ddir) {   // explicitly rounded products: a second use of the contractable ones above would keep them out of dmean's FMAs
+        ddir[0] = LGR_MUL((s2 - ox * ox) * ddx - oy * ox * ddy - oz * ox * ddz, inv32);
+        ddir[1] = LGR_MUL(-ox * oy * ddx + (s2 - oy * oy) * ddy - oz * oy * ddz, inv32);
+        ddir[2] = LGR_MUL(-ox * oz * ddx - oy * oz * ddy + (s2 - oz * oz) * ddz, inv32);
+    }
 }
 
 // dL/dSigma (6, doubled off-diagonals) -> dL/d(mod*scale) and dL/dquaternion

@@ -334,20 +334,95 @@ struct RawDepth {
     int mode;         // 0 = alpha only (word 9 is zero), 1 = z, 2 = inverse
 };
 
-__device__ __forceinline__ void depth_grad_to_mean(const RawDepth& dz, const float* __restrict__ rec, size_t i, const float* view, float* dmean)
+// dL/dz of Gaussian i from its accumulator record (word 9 = dL/d(depth value))
+__device__ __forceinline__ float depth_grad_z(const RawDepth& dz, const float* __restrict__ rec, size_t i)
 {
     float g = rec[9];
     if (dz.mode == 2) {
         const float r = __frcp_rn(dz.z[i]);
         g = -(g * r) * r;
     }
+    return g;
+}
+
+__device__ __forceinline__ void depth_grad_to_mean(const RawDepth& dz, const float* __restrict__ rec, size_t i, const float* view, float* dmean)
+{
+    const float g = depth_grad_z(dz, rec, i);
     dmean[0] = fmaf(g, view[2], dmean[0]);
     dmean[1] = fmaf(g, view[6], dmean[1]);
     dmean[2] = fmaf(g, view[10], dmean[2]);
 }
 
-template <bool DEPTH>
-__device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& a, const RawDepth& dz)
+// ---- camera gradients (lgr_backward_raw_camera, DESIGN.md section 7) ----
+// Each differentiated Gaussian contributes 27 live terms:
+//   [3r + k]       dL/dV[4r + k]       r = 0..3, k = 0..2   (V = viewmatrix; V[4r + 3] is never read)
+//   [12 + 3r + k]  dL/dPm[4r + c_k]    c = (0, 1, 3)        (Pm = projmatrix; Pm[4r + 2] is never read)
+//   [24 + c]       dL/dcampos[c]
+// A warp sums its lanes' terms with a fixed butterfly, the warps of a block add theirs in warp order in shared memory, and the block
+// writes one 27-float row (entry k of block b at rows[k * gridDim.x + b]); camera_grad_finish_kernel adds the rows.  No float atomics.
+constexpr int CAM_TERMS = 27;
+
+// dcam: cov2d_backward's camera output (dL/dt incl. any depth-plane dL/dz, then the T = J W term); dh: mean2d_backward's; ddir:
+// sh_backward's view-direction term.  p = (x, y, z, 1) is the world mean.
+__device__ __forceinline__ void cam_terms(const float* dcam, const float* dh, const float* ddir, float x, float y, float z, float* t)
+{
+    const float p[4] = {x, y, z, 1.f};
+#pragma unroll
+    for (int r = 0; r < 4; r++)
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            t[3 * r + k] = r < 3 ? fmaf(p[r], dcam[k], dcam[3 + 3 * r + k]) : dcam[k];
+            t[12 + 3 * r + k] = p[r] * dh[k];
+        }
+    t[24] = -ddir[0]; t[25] = -ddir[1]; t[26] = -ddir[2];
+}
+
+// the warp's sum of t[] into lane 0's `acc` row (acc += sum); every lane must call it
+__device__ __forceinline__ void cam_warp_add(float* t, float* acc, int lane)
+{
+#pragma unroll
+    for (int k = 0; k < CAM_TERMS; k++) {
+        float s = t[k];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(FULL, s, off);
+        if (lane == 0) acc[k] += s;
+    }
+}
+
+// after a __syncthreads: entry k of this block's row = sum over the block's warps, in warp order
+__device__ __forceinline__ void cam_block_row(const float* part, int nwarps, float* rows)
+{
+    if (threadIdx.x < CAM_TERMS) {
+        float s = part[threadIdx.x];
+        for (int w = 1; w < nwarps; w++) s += part[w * CAM_TERMS + threadIdx.x];
+        rows[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = s;
+    }
+}
+
+// dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3] from `nrows` block rows: warp k adds entry k, lane l the rows l, l + 32, ...
+// in order, then a fixed butterfly -- the same order for every run with the same rows.  The eight unread entries are written as 0.
+__global__ void __launch_bounds__(1024) camera_grad_finish_kernel(const float* __restrict__ rows, int nrows, float* __restrict__ dview,
+                                                                  float* __restrict__ dproj, float* __restrict__ dcampos)
+{
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp < CAM_TERMS) {
+        float s = 0.f;
+        for (int b = lane; b < nrows; b += 32) s += rows[(size_t)warp * nrows + b];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(FULL, s, off);
+        if (lane == 0) {
+            if (warp < 12) dview[4 * (warp / 3) + warp % 3] = s;
+            else if (warp < 24) dproj[4 * ((warp - 12) / 3) + ((warp - 12) % 3 == 2 ? 3 : (warp - 12) % 3)] = s;
+            else dcampos[warp - 24] = s;
+        }
+    } else if (warp == CAM_TERMS && lane < 8) {
+        if (lane < 4) dview[4 * lane + 3] = 0.f;
+        else dproj[4 * (lane - 4) + 2] = 0.f;
+    }
+}
+
+template <bool DEPTH, bool CAM = false>
+__device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& a, const RawDepth& dz, float* cam_part = nullptr)
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
     const int nrest = (a.M - 1) * 3;
@@ -359,6 +434,7 @@ __device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& 
     if (threadIdx.x < 16) s_cam[threadIdx.x] = a.view[threadIdx.x];
     else if (threadIdx.x < 32) s_cam[threadIdx.x] = a.proj[threadIdx.x - 16];
     else if (threadIdx.x < 35) s_cam[threadIdx.x] = a.campos[threadIdx.x - 32];
+    if (CAM && threadIdx.x < 8 * CAM_TERMS) cam_part[threadIdx.x] = 0.f;   // warps that have no Gaussian add nothing
     if (lane == 0) {
         mbar_init(&bars[warp], 1);
         fence_mbar_init();
@@ -399,6 +475,9 @@ __device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& 
     float dmean[3] = {0.f, 0.f, 0.f}, dscale[3] = {0.f, 0.f, 0.f}, dq[4] = {0.f, 0.f, 0.f, 0.f};
     float dop = 0.f, g2x = 0.f, g2y = 0.f, dRGB[3] = {0.f, 0.f, 0.f};
     float x = 0.f, y = 0.f, z = 0.f;
+    float cin[CAM ? 18 : 1];   // CAM: cov2d_backward's 12 camera values, mean2d_backward's 3, sh_backward's 3 (zero when not differentiated)
+#pragma unroll
+    for (int k = 0; k < (CAM ? 18 : 1); k++) cin[k] = 0.f;
     if (vis) {
         const float4 co = a.conic_opacity[si];
         const Grad2D g2 = accum_to_grad2d(a.acc + si * ACC_STRIDE, co, a.W, a.H);
@@ -406,9 +485,10 @@ __device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& 
         float c3[6], dcov[6];
 #pragma unroll
         for (int k = 0; k < 6; k++) c3[k] = a.cov3D[6 * si + k];
-        lgr::cov2d_backward(x, y, z, view, c3, a.fx, a.fy, a.tanx, a.tany, g2.dcx, g2.dcy, g2.dcw, dcov, dmean);
-        lgr::mean2d_backward(x, y, z, proj, g2.dm2x, g2.dm2y, dmean);
+        lgr::cov2d_backward(x, y, z, view, c3, a.fx, a.fy, a.tanx, a.tany, g2.dcx, g2.dcy, g2.dcw, dcov, dmean, CAM ? cin : nullptr);
+        lgr::mean2d_backward(x, y, z, proj, g2.dm2x, g2.dm2y, dmean, CAM ? cin + 12 : nullptr);
         if (DEPTH) depth_grad_to_mean(dz, a.acc + si * ACC_STRIDE, si, view, dmean);
+        if (CAM && DEPTH) cin[2] += depth_grad_z(dz, a.acc + si * ACC_STRIDE, si);   // z = t_2
         g2x = g2.dm2x; g2y = g2.dm2y;
         const unsigned cb = a.clamped[i];
         dRGB[0] = (cb & 1u) ? 0.f : g2.dcol[0]; dRGB[1] = (cb & 2u) ? 0.f : g2.dcol[1]; dRGB[2] = (cb & 4u) ? 0.f : g2.dcol[2];
@@ -445,14 +525,14 @@ __device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& 
                                      if (k == 0) dd[c] = val;
                                      else rr[3 * (k - 1) + c] = val;
                                  },
-                                 x, y, z, cam, dRGB, dmean);
+                                 x, y, z, cam, dRGB, dmean, CAM ? cin + 15 : nullptr);
             } else if (a.D > 0) {
                 lgr::sh_backward(a.D, [&](int k) { return k < 3 ? dd[k] : rr[k - 3]; },
                                  [&](int k, int c, float val) {
                                      if (k == 0) dd[c] = val;
                                      else rr[3 * (k - 1) + c] = val;
                                  },
-                                 x, y, z, cam, dRGB, dmean);
+                                 x, y, z, cam, dRGB, dmean, CAM ? cin + 15 : nullptr);
             } else {
 #pragma unroll
                 for (int c = 0; c < 3; c++) dd[c] = LGR_C0 * dRGB[c];
@@ -471,6 +551,11 @@ __device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& 
         if (a.d_rgb) {
             a.d_rgb[3 * si] = dRGB[0]; a.d_rgb[3 * si + 1] = dRGB[1]; a.d_rgb[3 * si + 2] = dRGB[2];
         }
+    }
+    if (CAM) {
+        float t[CAM_TERMS];
+        cam_terms(cin, cin + 12, cin + 15, x, y, z, t);
+        cam_warp_add(t, cam_part + warp * CAM_TERMS, lane);
     }
     if (a.d_rest == nullptr) return;  // compact mode: the SH gradient is rebuilt from d_rgb (sh_grad_from_views_kernel)
     __syncwarp();
@@ -491,6 +576,24 @@ __device__ __forceinline__ void preprocess_backward_raw_body(const RawBackArgs& 
 
 __global__ void __launch_bounds__(256) preprocess_backward_raw_kernel(RawBackArgs a) { preprocess_backward_raw_body<false>(a, RawDepth{}); }
 __global__ void __launch_bounds__(256) preprocess_backward_raw_depth_kernel(RawBackArgs a, RawDepth dz) { preprocess_backward_raw_body<true>(a, dz); }
+
+// the dense kernels plus one camera-gradient row per block (rows: [27][gridDim.x])
+template <bool DEPTH>
+__device__ __forceinline__ void preprocess_backward_raw_cam_body(const RawBackArgs& a, const RawDepth& dz, float* __restrict__ cam_rows)
+{
+    __shared__ float part[8 * CAM_TERMS];
+    preprocess_backward_raw_body<DEPTH, true>(a, dz, part);
+    __syncthreads();
+    cam_block_row(part, 8, cam_rows);
+}
+__global__ void __launch_bounds__(256) preprocess_backward_raw_cam_kernel(RawBackArgs a, float* cam_rows)
+{
+    preprocess_backward_raw_cam_body<false>(a, RawDepth{}, cam_rows);
+}
+__global__ void __launch_bounds__(256) preprocess_backward_raw_depth_cam_kernel(RawBackArgs a, RawDepth dz, float* cam_rows)
+{
+    preprocess_backward_raw_cam_body<true>(a, dz, cam_rows);
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // View-parallel SH gradient.  For one view dL/dSH[k][c] = basis_k(dir) * dRGB[c] is rank-1 per Gaussian

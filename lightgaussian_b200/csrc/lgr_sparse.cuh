@@ -478,9 +478,11 @@ __global__ void __launch_bounds__(256) kback_zero_flag_depth_kernel(KbackZeroArg
 constexpr int KC_THREADS = 128;   // compacted K7+K8: 4 warps per block
 constexpr int KC_ROW = 49;        // floats per staged SH row (48 + 1: conflict-free at one row per lane)
 
-template <bool DEPTH>
+// CAM: also the camera-gradient terms (lgr_raw.cuh, cam_terms); each warp adds its per-iteration sums into its own row of the shared
+// cam_acc ([4][27]) across the grid-stride loop, not in 27 more registers per lane
+template <bool DEPTH, bool CAM = false>
 __device__ __forceinline__ void preprocess_backward_compact_body(const RawBackArgs& a, const int* __restrict__ idx, const int* __restrict__ counter,
-                                                                 const RawDepth& dz)
+                                                                 const RawDepth& dz, float* cam_acc = nullptr)
 {
     // SH rows (48 floats per Gaussian) are scattered in memory: each warp moves its 32 rows through shared memory with row-contiguous
     // accesses (2 + 1 instructions per row) instead of 48 strided ones per lane -- 8x fewer sectors touched for the loads and the stores
@@ -489,6 +491,7 @@ __device__ __forceinline__ void preprocess_backward_compact_body(const RawBackAr
     if (threadIdx.x < 16) s_cam[threadIdx.x] = a.view[threadIdx.x];
     else if (threadIdx.x < 32) s_cam[threadIdx.x] = a.proj[threadIdx.x - 16];
     else if (threadIdx.x < 35) s_cam[threadIdx.x] = a.campos[threadIdx.x - 32];
+    if (CAM && threadIdx.x < KC_THREADS / 32 * CAM_TERMS) cam_acc[threadIdx.x] = 0.f;
     __syncthreads();
     const float* view = s_cam;
     const float* proj = s_cam + 16;
@@ -531,17 +534,23 @@ __device__ __forceinline__ void preprocess_backward_compact_body(const RawBackAr
             __syncwarp();
         }
         float* mine = rows + lane * KC_ROW;
+        float cin[CAM ? 18 : 1];   // as in preprocess_backward_raw_body
+        float px = 0.f, py = 0.f, pz = 0.f;
+#pragma unroll
+        for (int k = 0; k < (CAM ? 18 : 1); k++) cin[k] = 0.f;
         if (valid) {
             float dmean[3] = {0.f, 0.f, 0.f}, dscale[3], dq[4], dRGB[3];
             const float4 co = a.conic_opacity[si];
             const Grad2D g2 = accum_to_grad2d(a.acc + si * ACC_STRIDE, co, a.W, a.H);
             const float x = a.xyz[3 * si], y = a.xyz[3 * si + 1], z = a.xyz[3 * si + 2];
+            if (CAM) { px = x; py = y; pz = z; }
             float c3[6], dcov[6];
 #pragma unroll
             for (int k = 0; k < 6; k++) c3[k] = a.cov3D[6 * si + k];
-            lgr::cov2d_backward(x, y, z, view, c3, a.fx, a.fy, a.tanx, a.tany, g2.dcx, g2.dcy, g2.dcw, dcov, dmean);
-            lgr::mean2d_backward(x, y, z, proj, g2.dm2x, g2.dm2y, dmean);
+            lgr::cov2d_backward(x, y, z, view, c3, a.fx, a.fy, a.tanx, a.tany, g2.dcx, g2.dcy, g2.dcw, dcov, dmean, CAM ? cin : nullptr);
+            lgr::mean2d_backward(x, y, z, proj, g2.dm2x, g2.dm2y, dmean, CAM ? cin + 12 : nullptr);
             if (DEPTH) depth_grad_to_mean(dz, a.acc + si * ACC_STRIDE, si, view, dmean);
+            if (CAM && DEPTH) cin[2] += depth_grad_z(dz, a.acc + si * ACC_STRIDE, si);
             const unsigned cb = a.clamped[i];
             dRGB[0] = (cb & 1u) ? 0.f : g2.dcol[0]; dRGB[1] = (cb & 2u) ? 0.f : g2.dcol[1]; dRGB[2] = (cb & 4u) ? 0.f : g2.dcol[2];
             const float s0 = act_exp(a.scaling[3 * si]), s1 = act_exp(a.scaling[3 * si + 1]), s2 = act_exp(a.scaling[3 * si + 2]);
@@ -558,7 +567,8 @@ __device__ __forceinline__ void preprocess_backward_compact_body(const RawBackAr
             const float o = co.w;
             const float dop = (g2.dop * (1.0f - o)) * o;
             if (a.D > 0) {   // coefficients in, gradient out, in place in the lane's staged row
-                lgr::sh_backward(a.D, [&](int k) { return mine[k]; }, [&](int k, int c, float val) { mine[3 * k + c] = val; }, x, y, z, cam, dRGB, dmean);
+                lgr::sh_backward(a.D, [&](int k) { return mine[k]; }, [&](int k, int c, float val) { mine[3 * k + c] = val; }, x, y, z, cam, dRGB, dmean,
+                                 CAM ? cin + 15 : nullptr);
             } else {
 #pragma unroll
                 for (int c = 0; c < 3; c++) mine[c] = LGR_C0 * dRGB[c];
@@ -571,6 +581,11 @@ __device__ __forceinline__ void preprocess_backward_compact_body(const RawBackAr
             if (a.d_rgb) {
                 a.d_rgb[3 * si] = dRGB[0]; a.d_rgb[3 * si + 1] = dRGB[1]; a.d_rgb[3 * si + 2] = dRGB[2];
             }
+        }
+        if (CAM) {
+            float t[CAM_TERMS];
+            cam_terms(cin, cin + 12, cin + 15, px, py, pz, t);
+            cam_warp_add(t, cam_acc + warp * CAM_TERMS, lane);
         }
         __syncwarp();
         // gradient rows out (the rows were zero-filled: only the active degrees are written)
@@ -595,6 +610,27 @@ __global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_depth_
                                                                                         const int* __restrict__ counter, RawDepth dz)
 {
     preprocess_backward_compact_body<true>(a, idx, counter, dz);
+}
+// the compacted kernels plus one camera-gradient row per block (cam_rows: [27][gridDim.x])
+template <bool DEPTH>
+__device__ __forceinline__ void preprocess_backward_compact_cam_body(const RawBackArgs& a, const int* __restrict__ idx, const int* __restrict__ counter,
+                                                                     const RawDepth& dz, float* __restrict__ cam_rows)
+{
+    __shared__ float acc[KC_THREADS / 32 * CAM_TERMS];
+    preprocess_backward_compact_body<DEPTH, true>(a, idx, counter, dz, acc);
+    __syncthreads();
+    cam_block_row(acc, KC_THREADS / 32, cam_rows);
+}
+__global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_cam_kernel(RawBackArgs a, const int* __restrict__ idx,
+                                                                                      const int* __restrict__ counter, float* __restrict__ cam_rows)
+{
+    preprocess_backward_compact_cam_body<false>(a, idx, counter, RawDepth{}, cam_rows);
+}
+__global__ void __launch_bounds__(KC_THREADS) preprocess_backward_compact_depth_cam_kernel(RawBackArgs a, const int* __restrict__ idx,
+                                                                                            const int* __restrict__ counter, RawDepth dz,
+                                                                                            float* __restrict__ cam_rows)
+{
+    preprocess_backward_compact_cam_body<true>(a, idx, counter, dz, cam_rows);
 }
 
 }  // namespace

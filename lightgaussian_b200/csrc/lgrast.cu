@@ -65,14 +65,15 @@ std::atomic<uint64_t> g_launches{0};
 
 // ---- optional per-stage device timing (CUDA events on the launch stream), used by bench.py's roofline ----
 enum StageId { ST_PREPROCESS = 0, ST_DEPTH_SORT, ST_SCAN, ST_EMIT, ST_TILE_SORT, ST_RANGES, ST_BLEND_FWD, ST_BLEND_FWD_COUNT,
-               ST_SCORE, ST_BLEND_BWD, ST_PREPROCESS_BWD, ST_MEMSET, ST_SH_GRAD, ST_PEER_ALLREDUCE, ST_LOSS_FWD, ST_LOSS_BWD, ST_ADAMW, ST_COMPACT, ST_VQ_ASSIGN, ST_VQ_UPDATE, ST_SPARSE_PACK, ST_SPARSE_ACC, ST_BIN_DSORT, ST_BIN_COUNT, ST_BIN_SCATTER, ST_DET_GATHER, ST_ADAMW_SELECTIVE, ST_COUNT };
+               ST_SCORE, ST_BLEND_BWD, ST_PREPROCESS_BWD, ST_MEMSET, ST_SH_GRAD, ST_PEER_ALLREDUCE, ST_LOSS_FWD, ST_LOSS_BWD, ST_ADAMW, ST_COMPACT, ST_VQ_ASSIGN, ST_VQ_UPDATE, ST_SPARSE_PACK, ST_SPARSE_ACC, ST_BIN_DSORT, ST_BIN_COUNT, ST_BIN_SCATTER, ST_DET_GATHER, ST_ADAMW_SELECTIVE, ST_CAMERA_FINISH, ST_COUNT };
 const char* const kStageNames[ST_COUNT] = {"preprocess_kernel", "depth_sort(cub)", "scan(cub)", "emit_kernel", "tile_sort(cub)",
                                            "ranges_kernel", "blend_forward_kernel", "blend_forward_kernel<count>", "score_kernel",
                                            "blend_backward_kernel", "preprocess_backward_kernel", "memset", "sh_grad_from_views_kernel",
                                            "peer_allreduce_kernel", "image_loss_forward_kernel", "image_loss_backward_kernel", "adamw_multi_kernel",
                                            "compact_gather_kernel", "vq_assign_kernel", "vq_ema_kernels", "sparse_pack(flag+scan+index+K8)",
                                            "sparse_accumulate_kernel", "depth_sort(dsort_count+bin_scan+dsort_scatter x3)", "tile_count_kernel+bin_scan_kernel",
-                                           "tile_scatter_kernel", "det_gather_kernel", "adamw_selective_kernel"};
+                                           "tile_scatter_kernel", "det_gather_kernel", "adamw_selective_kernel",
+                                           "camera_grad_finish_kernel"};
 struct ProfRecord { int stage; cudaEvent_t a, b; };
 bool g_prof_on = false;
 std::vector<ProfRecord> g_prof_records;
@@ -1996,10 +1997,20 @@ int lgr_backward_raw_end(const lgr_view* v, int P, int M, const lgr_raw_params* 
     return lgr_backward_raw_end_range(v, P, M, params, radii, geometry_blob, grads, dL_dmeans2D, 0, P, cuda_stream);
 }
 
+// camera gradients of one backward (lgr_backward_raw_camera): K7+K8 writes one 27-float row per block into `rows` ([27][nrows]) and
+// records how many it wrote; a call that launches no K7+K8 leaves nrows at 0
+struct CamGrad {
+    float* rows;
+    int nrows;
+};
+
 // the same for Gaussians [first, first+count) only; first must be a multiple of 256.  Lets the caller start exchanging the gradients
-// of one range while the next range is still being computed.  rd: the depth variant of K7+K8 (lgr_backward_raw_depth, whole view)
+// of one range while the next range is still being computed.  rd: the depth variant of K7+K8 (lgr_backward_raw_depth, whole view).
+// cg: the camera variant of K7+K8 (lgr_backward_raw_camera, whole view); in deterministic mode it takes the dense kernel, whose block
+// rows follow the Gaussian index order
 static int backward_raw_end_impl(const lgr_view* v, int P, int M, const lgr_raw_params* params, const int32_t* radii, char* geometry_blob,
-                                 const lgr_raw_grads* grads, float* dL_dmeans2D, int first, int count, void* cuda_stream, const RawDepth* rd)
+                                 const lgr_raw_grads* grads, float* dL_dmeans2D, int first, int count, void* cuda_stream, const RawDepth* rd,
+                                 CamGrad* cg = nullptr)
 {
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
     if (P == 0 || count == 0) return LGR_OK;
@@ -2043,7 +2054,7 @@ static int backward_raw_end_impl(const lgr_view* v, int P, int M, const lgr_raw_
     if (compact) { a.d_rest = nullptr; a.d_dc = nullptr; }
     const bool rows_zeroed = t_rows_zeroed;
     t_rows_zeroed = false;
-    if (!compact && first == 0 && count == P && g_kback_mode != 1) {
+    if (!compact && first == 0 && count == P && g_kback_mode != 1 && !(cg && g_det)) {
         // whole view, dense outputs: zero-fill (unless the blend backward already did it) + flag, then K7+K8 on the compacted list of
         // Gaussians with a non-zero gradient (lgr_sparse.cuh).  The id list reuses sorted_ids (dead after the forward's binning), the
         // count a header word.
@@ -2062,7 +2073,15 @@ static int backward_raw_end_impl(const lgr_view* v, int P, int M, const lgr_raw_
         LGR_LAUNCH_CHECK("kback_zero_flag_kernel", debug, stream);
         a.P = P;
         const int blocks = std::min((P + KC_THREADS - 1) / KC_THREADS, LGR_SMS * 8);
-        if (rd)
+        if (cg) {
+            cg->nrows = blocks;
+            if (rd)
+                preprocess_backward_compact_depth_cam_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter,
+                                                                                                *rd, cg->rows);
+            else
+                preprocess_backward_compact_cam_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter,
+                                                                                          cg->rows);
+        } else if (rd)
             preprocess_backward_compact_depth_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter, *rd);
         else
             preprocess_backward_compact_kernel<<<blocks, KC_THREADS, 0, stream>>>(a, reinterpret_cast<const int*>(geo.sorted_ids), counter);
@@ -2070,7 +2089,18 @@ static int backward_raw_end_impl(const lgr_view* v, int P, int M, const lgr_raw_
         return LGR_OK;
     }
     const size_t smem = raw_smem_bytes(M);
-    if (rd) {
+    if (cg) {
+        const int blocks = (count + 255) / 256;
+        cg->nrows = blocks;
+        ProfScope ps(ST_PREPROCESS_BWD, stream);
+        if (rd) {
+            LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_backward_raw_depth_cam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            preprocess_backward_raw_depth_cam_kernel<<<blocks, 256, smem, stream>>>(a, *rd, cg->rows);
+        } else {
+            LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_backward_raw_cam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            preprocess_backward_raw_cam_kernel<<<blocks, 256, smem, stream>>>(a, cg->rows);
+        }
+    } else if (rd) {
         LGR_CUDA_TRY(cudaFuncSetAttribute(preprocess_backward_raw_depth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ProfScope ps(ST_PREPROCESS_BWD, stream);
         preprocess_backward_raw_depth_kernel<<<(count + 255) / 256, 256, smem, stream>>>(a, *rd);
@@ -2091,7 +2121,8 @@ int lgr_backward_raw_end_range(const lgr_view* v, int P, int M, const lgr_raw_pa
 
 static int backward_raw_impl(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
                              char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, const lgr_raw_grads* grads,
-                             float* dL_dmeans2D, void* cuda_stream, const BlendDepthBack* db, const RawDepth* rd, float* absgrad = nullptr)
+                             float* dL_dmeans2D, void* cuda_stream, const BlendDepthBack* db, const RawDepth* rd, float* absgrad = nullptr,
+                             CamGrad* cg = nullptr)
 {
     t_zero_req.P = 0;
     t_rows_zeroed = false;
@@ -2109,7 +2140,7 @@ static int backward_raw_impl(const lgr_view* v, int P, int M, int num_rendered, 
                                            absgrad);
     t_zero_req.P = 0;
     if (st != LGR_OK) { t_rows_zeroed = false; return st; }
-    return backward_raw_end_impl(v, P, M, params, radii, geometry_blob, grads, dL_dmeans2D, 0, P, cuda_stream, rd);
+    return backward_raw_end_impl(v, P, M, params, radii, geometry_blob, grads, dL_dmeans2D, 0, P, cuda_stream, rd, cg);
 }
 
 int lgr_backward_raw(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
@@ -2206,6 +2237,52 @@ int lgr_backward_raw_absgrad(const lgr_view* v, int P, int M, int num_rendered, 
     }
     return backward_raw_impl(v, P, M, num_rendered, params, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dmeans2D,
                              cuda_stream, nullptr, nullptr, num_rendered > 0 ? dL_dmeans2D_abs : nullptr);
+}
+
+// ---- camera gradients (DESIGN section 7) ----
+// block rows of the larger of the two K7+K8 grids: the dense kernel's (one block per 256 Gaussians) and the compacted kernel's
+size_t lgr_camera_grad_workspace_bytes(int P)
+{
+    if (P <= 0) return 256;
+    const size_t rows = (size_t)std::max((P + 255) / 256, std::min((P + KC_THREADS - 1) / KC_THREADS, LGR_SMS * 8));
+    return align_up(rows * CAM_TERMS * sizeof(float), 256);
+}
+
+int lgr_backward_raw_camera(const lgr_view* v, int P, int M, int num_rendered, const lgr_raw_params* params, const int32_t* radii,
+                            char* geometry_blob, char* binning_blob, char* image_blob, const float* dL_dout_color, int depth_mode,
+                            const float* dL_ddepth, const float* dL_dalpha, const lgr_raw_grads* grads, float* dL_dmeans2D,
+                            float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, void* workspace, size_t workspace_bytes,
+                            void* cuda_stream)
+{
+    const bool planes = dL_ddepth || dL_dalpha;
+    if (planes && !depth_request_ok("lgr_backward_raw_camera", depth_mode, dL_ddepth != nullptr)) return LGR_ERR_INVALID_ARG;
+    if (P < 0 || !dL_dviewmatrix || !dL_dprojmatrix || !dL_dcampos || !workspace || workspace_bytes < lgr_camera_grad_workspace_bytes(P) ||
+        ((uintptr_t)workspace & 3)) {
+        g_last_error = "lgr_backward_raw_camera: the three camera outputs and a 4-byte aligned workspace of lgr_camera_grad_workspace_bytes(P) "
+                       "bytes are required";
+        return LGR_ERR_INVALID_ARG;
+    }
+    if (planes && P > 0 && !geometry_blob) {
+        g_last_error = "lgr_backward_raw_camera: missing required argument";
+        return LGR_ERR_INVALID_ARG;
+    }
+    BlendDepthBack db = {};
+    RawDepth rd = {};
+    if (planes && P > 0) {
+        db = {dL_ddepth, dL_dalpha, 1 + depth_mode, P};
+        rd = {carve_geometry(geometry_blob, (size_t)P, false).depth, depth_mode};
+    }
+    CamGrad cg = {static_cast<float*>(workspace), 0};
+    const int st = backward_raw_impl(v, P, M, num_rendered, params, radii, geometry_blob, binning_blob, image_blob, dL_dout_color, grads,
+                                     dL_dmeans2D, cuda_stream, planes ? &db : nullptr, planes ? &rd : nullptr, nullptr, &cg);
+    if (st != LGR_OK) return st;
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    {
+        ProfScope ps(ST_CAMERA_FINISH, stream);
+        camera_grad_finish_kernel<<<1, 1024, 0, stream>>>(cg.rows, cg.nrows, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos);
+    }
+    LGR_LAUNCH_CHECK("camera_grad_finish_kernel", v && v->debug != 0, stream);
+    return LGR_OK;
 }
 
 // ---- sparse view-parallel exchange (lgr_sparse.cuh) ----

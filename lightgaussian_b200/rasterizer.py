@@ -605,11 +605,15 @@ def depth_alpha_refusal() -> str | None:
 
 
 class _RasterizeRawLeavesDepth(torch.autograd.Function):
-    """render(depth=..., alpha=...)'s node: _RasterizeRawLeaves plus the depth and alpha planes ([1,H,W] each; an empty placeholder
-    for one that was not asked for).  The backward takes the existing lgr_backward_raw when neither plane received a gradient."""
+    """render(depth=..., alpha=..., camera_grad=...)'s node: _RasterizeRawLeaves plus the depth and alpha planes ([1,H,W] each; an empty
+    placeholder for one that was not asked for) and, as optional tensor inputs, the three camera tensors the raster settings carry
+    (viewmatrix, projmatrix, campos; None unless camera gradients are asked for).  With no plane its forward is lgr_forward_raw.  The
+    backward takes lgr_backward_raw_camera when a camera tensor needs a gradient, else the existing lgr_backward_raw when neither plane
+    received a gradient, else lgr_backward_raw_depth."""
 
     @staticmethod
-    def forward(ctx, xyz, means2D, dc, rest, scaling, rotation, opacity, raster_settings, depth_mode, want_depth, want_alpha):
+    def forward(ctx, xyz, means2D, dc, rest, scaling, rotation, opacity, raster_settings, depth_mode, want_depth, want_alpha,
+                viewmatrix=None, projmatrix=None, campos=None):
         H, W = int(raster_settings.image_height), int(raster_settings.image_width)
         plane = lambda on: torch.empty((1, H, W), dtype=torch.float32, device=xyz.device) if on else None  # noqa: E731
         out_depth, out_alpha = plane(want_depth), plane(want_alpha)
@@ -618,6 +622,7 @@ class _RasterizeRawLeavesDepth(torch.autograd.Function):
         ctx.raster_settings = raster_settings
         ctx.num_rendered = R
         ctx.depth_mode = depth_mode
+        ctx.deterministic = _last_deterministic[0]
         ctx.save_for_backward(*leaves, radii, geom, binning, img)
         ctx.set_materialize_grads(False)
         empty = lambda: torch.empty((0,), dtype=torch.float32, device=xyz.device)  # noqa: E731
@@ -634,6 +639,7 @@ class _RasterizeRawLeavesDepth(torch.autograd.Function):
     def backward(ctx, grad_out_color, _, grad_depth, grad_alpha):
         rs = ctx.raster_settings
         xyz, dc, rest, scaling, rotation, opacity, radii, geom, binning, img = ctx.saved_tensors
+        capi.set_deterministic(ctx.deterministic)   # the mode of the forward, whatever the flag says now
         H, W = int(rs.image_height), int(rs.image_width)
         if grad_out_color is None:
             grad_out_color = torch.zeros((3, H, W), dtype=torch.float32, device=xyz.device)
@@ -641,6 +647,13 @@ class _RasterizeRawLeavesDepth(torch.autograd.Function):
             grad_depth = None
         if grad_alpha is not None and grad_alpha.numel() == 0:
             grad_alpha = None
+        need_cam = ctx.needs_input_grad[11:14]
+        if any(need_cam):
+            trace.bump("raw_backward_camera")
+            g, g2d, cams = backward_raw_camera_native(rs, ctx.num_rendered, grad_out_color, ctx.depth_mode, grad_depth, grad_alpha, xyz, dc,
+                                                      rest, scaling, rotation, opacity, radii, geom, binning, img)
+            cam_grads = tuple(c if need else None for c, need in zip(cams, need_cam))
+            return (g[0], g2d, g[1], g[2], g[3], g[4], g[5], None, None, None, None) + cam_grads
         if grad_depth is None and grad_alpha is None:
             trace.bump("raw_backward_plain")
             g, g2d, _, _ = backward_raw_native(rs, ctx.num_rendered, grad_out_color, xyz, dc, rest, scaling, rotation, opacity, radii,
@@ -649,7 +662,7 @@ class _RasterizeRawLeavesDepth(torch.autograd.Function):
             trace.bump("raw_backward_depth")
             g, g2d = backward_raw_depth_native(rs, ctx.num_rendered, grad_out_color, ctx.depth_mode, grad_depth, grad_alpha, xyz, dc,
                                                rest, scaling, rotation, opacity, radii, geom, binning, img)
-        return g[0], g2d, g[1], g[2], g[3], g[4], g[5], None, None, None, None
+        return g[0], g2d, g[1], g[2], g[3], g[4], g[5], None, None, None, None, None, None, None
 
 
 def backward_raw_depth_native(rs, num_rendered, grad_out_color, depth_mode, grad_depth, grad_alpha, xyz, dc, rest, scaling, rotation,
@@ -676,20 +689,76 @@ def backward_raw_depth_native(rs, num_rendered, grad_out_color, depth_mode, grad
     return g, g2d
 
 
+def backward_raw_camera_native(rs, num_rendered, grad_out_color, depth_mode, grad_depth, grad_alpha, xyz, dc, rest, scaling, rotation,
+                               opacity, radii, geom, binning, img):
+    """lgr_backward_raw_camera: the six dense leaf gradients and dL/dmeans2D as backward_raw_depth_native, plus the camera gradients
+    (dL/dviewmatrix, dL/dprojmatrix, dL/dcampos) in the shapes of rs.viewmatrix, rs.projmatrix and rs.campos."""
+    lib = capi.load()
+    device = xyz.device
+    P, M = xyz.size(0), 1 + rest.size(1)
+    H, W = grad_out_color.size(1), grad_out_color.size(2)
+    g2d = torch.empty((P, 3), dtype=torch.float32, device=device)
+    g = [torch.empty(t.shape, dtype=torch.float32, device=device) for t in (xyz, dc, rest, scaling, rotation, opacity)]
+    dview = torch.empty((16,), dtype=torch.float32, device=device)
+    dproj = torch.empty((16,), dtype=torch.float32, device=device)
+    dcampos = torch.empty((3,), dtype=torch.float32, device=device)
+    ws_bytes = int(lib.lgr_camera_grad_workspace_bytes(P))
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
+    dpix = _f32c(grad_out_color, "grad_out_color")
+    gd = _f32c(grad_depth, "grad_depth") if grad_depth is not None else None
+    ga = _f32c(grad_alpha, "grad_alpha") if grad_alpha is not None else None
+    with torch.cuda.device(device):
+        view, keep = _make_view(device, rs.bg, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy, H, W,
+                                rs.scale_modifier, rs.sh_degree, False, rs.debug)
+        params, grads = _raw_struct(xyz, dc, rest, scaling, rotation, opacity), _raw_grads_struct(*g)
+        st = lib.lgr_backward_raw_camera(C.byref(view), P, M, int(num_rendered), C.byref(params), radii.data_ptr(), geom.data_ptr(),
+                                         binning.data_ptr(), img.data_ptr(), dpix.data_ptr(), int(depth_mode), capi.ptr(gd), capi.ptr(ga),
+                                         C.byref(grads), g2d.data_ptr(), dview.data_ptr(), dproj.data_ptr(), dcampos.data_ptr(),
+                                         ws.data_ptr(), ws_bytes, capi.current_stream_ptr(device))
+    capi.check(st, "lgr_backward_raw_camera")
+    cams = (dview.view(rs.viewmatrix.shape), dproj.view(rs.projmatrix.shape), dcampos.view(rs.campos.shape))
+    return g, g2d, cams
+
+
+def camera_grad_refusal(viewmatrix, projmatrix, campos) -> str | None:
+    """Why the fused node cannot return camera gradients for these camera tensors under the current settings, or None.  Checked
+    before any launch."""
+    if _exchange["world"] > 1:
+        return "the view-parallel gradient exchange has no camera gradients"
+    if _os.environ.get("LGR_SPARSE_SINGLE", "0") == "1":
+        return "LGR_SPARSE_SINGLE=1 (the sparse single-GPU backward) has no camera gradients"
+    for t, name, shape in ((viewmatrix, "world_view_transform", (4, 4)), (projmatrix, "full_proj_transform", (4, 4)),
+                           (campos, "camera_center", (3,))):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or tuple(t.shape) != shape:
+            what = f"{t.dtype} {'CUDA' if t.is_cuda else 'CPU'} {list(t.shape)}" if isinstance(t, torch.Tensor) else type(t).__name__
+            return f"the camera's {name} must be a float32 CUDA tensor of shape {list(shape)} (got {what})"
+    return None
+
+
 def rasterize_raw_leaves_depth(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity, raster_settings, depth=None,
-                               alpha=False):
+                               alpha=False, camera_grad=False):
     """(color, radii, depth, alpha) of the fused node: depth [1,H,W] when depth is "z" or "inverse" (else None), alpha [1,H,W] when
-    alpha (else None).  Raises RuntimeError before any launch where the settings have no depth or alpha output."""
+    alpha (else None).  camera_grad: raster_settings' viewmatrix, projmatrix and campos become tensor inputs of the node, so the ones
+    that require grad receive dL/d themselves (lgr_backward_raw_camera).  Raises RuntimeError before any launch where the settings
+    have no such output."""
+    planes = depth is not None or alpha
     if depth is not None and depth not in DEPTH_MODES:
         raise RuntimeError(f"depth={depth!r}: expected None, 'z' or 'inverse'")
     if raster_settings.f_count:
-        raise RuntimeError("depth / alpha: count mode (raster_settings.f_count) has no depth or alpha output")
+        raise RuntimeError("depth / alpha / camera_grad: count mode (raster_settings.f_count) has no depth, alpha or camera gradient")
     mode = DEPTH_MODES.get(depth, 0)
-    why = depth_alpha_refusal()
-    if why is not None:
-        raise RuntimeError(f"depth / alpha: {why}")
+    if planes:
+        why = depth_alpha_refusal()
+        if why is not None:
+            raise RuntimeError(f"depth / alpha: {why}")
+    cams = (None, None, None)
+    if camera_grad:
+        cams = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
+        why = camera_grad_refusal(*cams)
+        if why is not None:
+            raise RuntimeError(f"camera_grad: {why}")
     color, radii, d, a = _RasterizeRawLeavesDepth.apply(xyz, means2D, features_dc, features_rest, scaling, rotation, opacity,
-                                                        raster_settings, mode, depth is not None, bool(alpha))
+                                                        raster_settings, mode, depth is not None, bool(alpha), *cams)
     return color, radii, (d if depth is not None else None), (a if alpha else None)
 
 

@@ -20,7 +20,7 @@ from . import trace
 
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rasterize_raw_leaves, fused_activations_match_torch,
                          rest_row_stride, forward_vq_native, rasterize_raw_leaves_depth, depth_alpha_refusal, DEPTH_MODES,
-                         rasterize_raw_leaves_absgrad, absgrad_refusal)
+                         rasterize_raw_leaves_absgrad, absgrad_refusal, camera_grad_refusal)
 
 _LEAVES = ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")
 
@@ -152,10 +152,22 @@ def _unfused_reason(pc, pipe, override_color) -> str:
     return "a model without GaussianModel's raw float32 CUDA leaves and standard activations (exp / sigmoid / normalize)"
 
 
-def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, f_count, weight=False, depth=None, alpha=False):
+def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, f_count, weight=False, depth=None, alpha=False,
+            camera_grad=False):
     planes = depth is not None or alpha
     # LGR_DENSIFY_GRAD=abs: the training render's backward also produces viewspace_points.absgrad; checked before anything is read
     absgrad = not f_count and densify_grad_mode() == "abs" and torch.is_grad_enabled()
+    # camera_grad: the camera tensors become inputs of the fused node (only meaningful with gradients); checked before any launch
+    cam_grad = bool(camera_grad) and torch.is_grad_enabled()
+    if cam_grad:
+        if absgrad:
+            raise RuntimeError("render(camera_grad=True): LGR_DENSIFY_GRAD=abs has no camera gradients")
+        if not _can_fuse(pc, pipe, override_color):
+            raise RuntimeError(f"render(camera_grad=True) needs the fused path, which {_unfused_reason(pc, pipe, override_color)} rules out")
+        why = camera_grad_refusal(viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform,
+                                  viewpoint_camera.camera_center)
+        if why is not None:
+            raise RuntimeError(f"render(camera_grad=True): {why}")
     if absgrad:
         if planes:
             raise RuntimeError("LGR_DENSIFY_GRAD=abs cannot be combined with render(depth=..., alpha=...)")
@@ -204,10 +216,13 @@ def _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_col
         xyz_, dc, rest, scaling, rotation, opacity = _dense_leaves(pc)
         outputs = rasterize_raw_leaves_absgrad(xyz_, screenspace_points, dc, rest, scaling, rotation, opacity, settings)
         return _package(outputs, screenspace_points, f_count)
-    if planes:
-        trace.bump("render_depth_alpha")
+    if planes or cam_grad:
+        if planes:
+            trace.bump("render_depth_alpha")
+        if cam_grad:
+            trace.bump("render_camera_grad")
         color, radii, d, a = rasterize_raw_leaves_depth(pc._xyz, screenspace_points, pc._features_dc, pc._features_rest, pc._scaling,
-                                                        pc._rotation, pc._opacity, settings, depth, alpha)
+                                                        pc._rotation, pc._opacity, settings, depth, alpha, cam_grad)
         result = _package((color, radii), screenspace_points, False)
         if d is not None:
             result["depth"] = d
@@ -276,7 +291,8 @@ def _package(outputs, screenspace_points, f_count, blend_weight=None):
     return result
 
 
-def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None, *, depth=None, alpha=False):
+def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None, *, depth=None, alpha=False,
+           camera_grad=False):
     """Render the scene.  Background tensor (bg_color) must be on the GPU.
     depth="z" / "inverse" adds "depth", and alpha=True adds "alpha", to the result: [1,H,W] float32 planes with gradients to the
     leaves, sum_i alpha_i*T_i*z_i (z, or 1/z: view-space depth; background 0, not divided by alpha) and 1 - final T (DESIGN.md
@@ -285,8 +301,14 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     resident VQ model asked for them renders from its leaves, which materialise as on any call that needs them.
     With LGR_DENSIFY_GRAD=abs (read at each call) and gradients enabled, the backward also sets `viewspace_points.absgrad` ([P,2], the
     sum over pixels of each pixel's |dL/dmean2D| term, DESIGN.md section 7) for add_densification_stats; the same paths, depth= and
-    alpha= then raise RuntimeError before any launch.  Without gradients the variable changes nothing."""
-    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, False, depth=depth, alpha=alpha)
+    alpha= then raise RuntimeError before any launch.  Without gradients the variable changes nothing.
+    camera_grad=True (with gradients enabled) makes viewpoint_camera's world_view_transform, full_proj_transform and camera_center
+    tensor inputs of the fused node: those that require grad receive dL/d themselves in the backward (DESIGN.md section 7, "Camera
+    gradients"; the intrinsics get none).  It needs float32 CUDA tensors of shapes [4,4], [4,4], [3] and the fused path; the unfused
+    paths, LGR_DENSIFY_GRAD=abs, the view-parallel exchange and LGR_SPARSE_SINGLE=1 raise RuntimeError before any launch.  It works in
+    deterministic mode (bit-identical camera gradients run to run) and with depth= / alpha=.  Without gradients it changes nothing."""
+    return _render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, False, depth=depth, alpha=alpha,
+                   camera_grad=camera_grad)
 
 
 def count_render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):

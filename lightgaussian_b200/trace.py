@@ -12,6 +12,8 @@ took; with LGR_TRACE=<file> set, the counters below are written to that file (JS
     render_absgrad / raw_backward_absgrad  render() calls through the fused node that also computes the absolute-gradient
                                        densification statistic (LGR_DENSIFY_GRAD=abs) / its backwards (lgr_backward_raw_absgrad)
     densify_stats_absgrad              add_densification_stats calls that added ||absgrad|| (LGR_DENSIFY_GRAD=abs)
+    render_camera_grad / raw_backward_camera  render(camera_grad=True) calls with gradients enabled (the fused node with the camera
+                                       tensors as inputs) / its backwards through lgr_backward_raw_camera
 Cost when LGR_TRACE is unset: one dict increment per call."""
 from __future__ import annotations
 
